@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- CPD EM-iterations/sec at N = M = 100k 3-D points on N B200s (BASELINE.json metric).
+"""bench.py -- CPD EM-iterations/sec at N = M = 100k 3-D points on N H100s (BASELINE.json metric).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--points 100000]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--points 100000] [--dump-outputs DIR]
   N > 1 is launched by torchrun (one rank per GPU); rank 0 prints ONE JSON line.
 
 A "step" is one EM iteration (probreg/cpd.py:111-113: transform -> E-step -> M-step) of rigid CPD
@@ -19,6 +19,12 @@ targets are sharded over the ranks (one 32-double NCCL all-reduce per iteration)
             by, plus the HBM view (the kernel moves ~10 MB per iteration: P is never materialised).
   cpu_baseline / --impl reference: the oracle port of the reference's numpy path (oracle/cpd_oracle.py)
             on the host cores, on a bounded column sample of the same workload, extrapolated.
+  --dump-outputs DIR: after the timed steps, what the timed path computed in its last step as DIR/<name>.npy (float64):
+            the E-step arrays pt1, p1, px and the parameters of the rigid / affine step, or sigma2, W and the moved
+            source of the non-rigid step.  With more than one GPU only the parameters, which every rank receives whole
+            (pt1, p1 and px stay per rank).  An array of more than DUMP_ROWS rows is replaced by a fixed, seeded sample
+            of its rows, and the sampled row indices go to <name>_rows.npy: at most ~32 MB in all.  The inputs are
+            generated from fixed seeds, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -36,18 +42,18 @@ if ROOT not in sys.path:
 
 METRIC = "cpd_em_iterations_per_sec"
 UNIT = "it/s"
-FLOP_PER_PAIR_ITER = 29.0     # SURVEY 8(d): pass 1 = 3D+2 = 11, pass 2 = 5D+3 = 18 at D = 3
+FLOP_PER_PAIR_ITER = 29.0     # pass 1 = 3D+2 = 11, pass 2 = 5D+3 = 18 at D = 3
 
 
 def hbm_bytes_per_iter(n_local, m):
-    # SURVEY 8(d): algorithmic traffic of the fused E-step, per iteration and rank:
+    # algorithmic traffic of the fused E-step, per iteration and rank:
     # pass 1 reads 16 B/target + 16 B/source, writes 8 B/target; pass 2 reads 32 B/target + 16 B/source
     # and writes 32 B/source (p1, px in FP64).
     return 16 * n_local + 16 * m + 8 * n_local + 32 * n_local + 16 * m + 32 * m
 
 
 class ClockSampler(object):
-    """SM clocks / clock-event reasons while the job runs (B200_PROFILING.md recipe).  ONE poller (rank 0) for all the job's GPUs,
+    """SM clocks / clock-event reasons while the job runs.  ONE poller (rank 0) for all the job's GPUs,
     started before the warm-up.  NVML through pynvml, polled every 5 ms from a thread (a query costs microseconds, so even a
     140 ms timed region gets ~25 samples per GPU, and every sample has a timestamp: the median reported is over the samples that
     fall INTO the timed region); `nvidia-smi -lms 100` as the fallback when NVML cannot be loaded -- its samples are ~10x sparser
@@ -177,7 +183,7 @@ class ClockSampler(object):
 
 def workload(points, kind="rigid"):
     from probreg_b200.synthetic import synthetic_pair
-    if kind == "nonrigid":                      # SURVEY 8(d) config 5: the rigid generator's source + a smooth displacement
+    if kind == "nonrigid":                      # config 5: the rigid generator's source + a smooth displacement
         src, _ = synthetic_pair(points, "rigid")
         f = np.array([[1.0, 0.5, 0.0], [0.0, 1.0, 0.7], [0.3, 0.0, 1.0]])
         tgt = src + 0.03 * np.sin(2 * np.pi * src.dot(f)) + 0.002 * np.random.default_rng(9).standard_normal(src.shape)
@@ -186,8 +192,7 @@ def workload(points, kind="rigid"):
 
 
 # ---------------------------------------------------------------------------------------------
-# CPU arm: the UNMODIFIED reference (baseline/_ref/probreg, see baseline/install_ref.py) on a bounded sample;
-# the oracle port beside it as a second figure
+# CPU arm: the oracle port of the reference's numpy path on a bounded sample
 # ---------------------------------------------------------------------------------------------
 WORKLOADS = {
     2: ("rigid", 100000, "rigid CPD, synthetic 3-D N=M=%d, sigma2 auto, w=0, update_scale"),
@@ -209,50 +214,9 @@ def blas_threads():
         return int(os.cpu_count() or 1)
 
 
-def reference_sample(kind, points, cols, chunk=250):
-    """One EM iteration of the reference's own code (probreg/cpd.py:111-113) on `cols` of the `points` target columns:
-    Transformation.transform on all sources, CoherentPointDrift.expectation_step (cpd.py:71-88) column-chunked -- exact for
-    w = 0 because `den` is per column (SURVEY 8d) -- and the class's _maximization_step (cpd.py:160-192 / 219-244) on the sampled
-    columns' EstepResult.  The E-step time is extrapolated to all columns; the M-step and the transform are not (they cost
-    O(M + N), < 0.1 % of the iteration)."""
-    from baseline import ref_loader
-    rcpd, rtf = ref_loader.load()
-    from probreg_b200.synthetic import synthetic_pair
-    src, tgt = synthetic_pair(points, "affine" if kind == "affine" else "rigid")
-    cols = min(cols, points)
-    sub = tgt[:cols]
-    # sigma2_0 in closed form (the reference's _initialize would allocate an M x N float32 matrix: 40 GB at 100k)
-    s2 = float(((src * src).sum() / points + (tgt * tgt).sum() / points - 2.0 * src.mean(0).dot(tgt.mean(0))) / 3.0)
-    reg = rcpd.AffineCPD(src) if kind == "affine" else rcpd.RigidCPD(src, update_scale=True)
-    tfm = rtf.AffineTransformation(np.identity(3), np.zeros(3)) if kind == "affine" else rtf.RigidTransformation(np.identity(3), np.zeros(3))
-    # one untimed chunk first: the first M x chunk float64 temporaries of a process are page-faulted in (seconds in this
-    # image's sandbox), after which the allocator re-uses them -- the reference's steady state is what is timed
-    reg.expectation_step(src, sub[:chunk], s2, 0.0)
-    t0 = time.perf_counter()
-    ts = tfm.transform(src)
-    t_tf = time.perf_counter() - t0
-    t0 = time.perf_counter()
-    pt1, p1, px = [], np.zeros(points), np.zeros((points, 3))
-    for lo in range(0, cols, chunk):
-        es = reg.expectation_step(ts, sub[lo:lo + chunk], s2, 0.0)
-        pt1.append(es.pt1); p1 += es.p1; px += es.px
-    t_e = time.perf_counter() - t0
-    es = rcpd.EstepResult(np.concatenate(pt1), p1, px, float(p1.sum()))
-    t0 = time.perf_counter()
-    res = reg.maximization_step(sub, es, s2)
-    t_m = time.perf_counter() - t0
-    t_iter = t_e * (points / float(cols)) + t_m + t_tf
-    return {"value": 1.0 / t_iter, "unit": UNIT, "cores": blas_threads(), "host_cpus": os.cpu_count(), "kind": "reference",
-            "sample": "unmodified probreg/cpd.py (baseline/_ref): expectation_step on %d of %d target columns x all %d sources in "
-                      "chunks of %d (%.2f s, extrapolated x%.0f) + transform (%.3f s) + _maximization_step on the sampled "
-                      "columns (%.3f s); numpy/scipy as the reference uses them (~90%% single-threaded, BLAS threads = %d)"
-                      % (cols, points, points, chunk, t_e, points / float(cols), t_tf, t_m, blas_threads()),
-            "sec_per_iter_extrapolated": t_iter, "ns_per_pair": t_e / (cols * float(points)) * 1e9,
-            "sigma2_after": float(res.sigma2)}
-
-
 def port_sample(points, cols):
-    """The same iteration through the oracle port (oracle/cpd_oracle.py): a second CPU figure (about 3x faster than the reference)."""
+    """One EM iteration through the oracle port of the reference's numpy path (oracle/cpd_oracle.py), column-sampled and extrapolated
+    (exact for w = 0: `den` is per column)."""
     from oracle import cpd_oracle as orc
     src, tgt = workload(points)
     s2 = float(orc.sigma2_init_exact(src, tgt))
@@ -261,7 +225,7 @@ def port_sample(points, cols):
     orc.expectation_step(src, tgt[:chunk], s2, 0.0, n_global=points)          # untimed: see reference_sample
     t0 = time.perf_counter()
     ts = orc.apply_rigid(src, np.identity(3), np.zeros(3))
-    parts = [orc.expectation_step(ts, tgt[lo:lo + chunk], s2, 0.0, n_global=points) for lo in range(0, cols, chunk)]
+    parts = [orc.expectation_step(ts, tgt[lo:min(lo + chunk, cols)], s2, 0.0, n_global=points) for lo in range(0, cols, chunk)]
     es = orc.Estep(np.concatenate([e.pt1 for e in parts]), sum(e.p1 for e in parts), sum(e.px for e in parts),
                    float(sum(e.p1.sum() for e in parts)))
     t_e = time.perf_counter() - t0
@@ -275,16 +239,7 @@ def port_sample(points, cols):
 
 
 def cpu_sample(kind, points, cols):
-    """cpu_baseline of the bench line: the reference when baseline/_ref travelled with the repo, else the oracle port."""
-    from baseline import ref_loader
-    if ref_loader.available() and kind in ("rigid", "affine"):
-        out = reference_sample(kind, points, cols)
-        if kind == "rigid":
-            try:
-                out["port"] = port_sample(points, cols)
-            except Exception as e:          # noqa: BLE001
-                out["port"] = {"error": str(e)[:200]}
-        return out
+    """cpu_baseline of the bench line: the oracle port on the host cores."""
     out = port_sample(points, cols)
     out["cores"], out["host_cpus"] = blas_threads(), os.cpu_count()
     return out
@@ -407,6 +362,20 @@ def run_ours(args):
         total_ms = float(tt.item())
     ms_per_step = total_ms / args.steps
     value = 1e3 / ms_per_step
+    if args.dump_outputs:
+        pt1, p1, px, _ = h.last_estep()     # the E-step of the last timed iteration (this rank's share when world > 1)
+        # its parameters: the same iterations again from the same start (the EM loop is deterministic), the last one read back
+        reset()
+        for _ in range(3 + args.steps - 1):
+            h.em_step(read=False)
+        lin, t, scale, sigma2, q, n_p = h.em_step(read=True)
+        if not all(np.array_equal(a, b) for a, b in zip((pt1, p1, px), h.last_estep()[:3])):
+            raise SystemExit("--dump-outputs: the repeated iterations did not reproduce the timed ones")
+        if rank == 0:
+            out = {"lin": lin, "t": t, "scale": scale, "sigma2": sigma2, "q": q, "n_p": n_p}
+            if world == 1:
+                out.update(pt1=pt1, p1=p1, px=px)
+            dump_outputs(args.dump_outputs, out)
     final = h.em_step(read=True)            # the loop did real work: parameters moved towards the truth
 
     # ---- multi-rank runs: the sharded loop against the same iterations on ONE GPU (asserted, rank 0) ---------------
@@ -491,20 +460,12 @@ def run_ours(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-    hbm_src = "measured (MEASURED_PEAKS.json)" if "hbm_gbs" in peaks else "fallback (B200_PROFILING.md)"
+    hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
+    hbm_src = "measured (MEASURED_PEAKS.json)" if "hbm_gbs" in peaks else "H100 SXM data sheet (3.35 TB/s)"
     flops = FLOP_PER_PAIR_ITER * float(n_local) * float(n)
     ach_tf = flops / (t_estep_ms * 1e-3) / 1e12
-    nominal_tf = 2.0 * 128 * probe["sm_count"] * (clocks.get("sm_max_mhz") or 1965.0) * 1e6 / 1e12
+    nominal_tf = 2.0 * 128 * probe["sm_count"] * (clocks.get("sm_max_mhz") or 1980.0) * 1e6 / 1e12
     bytes_iter = hbm_bytes_per_iter(n_local, n)
-    traffic, traffic_src = None, None
-    try:   # dram__bytes_read.sum + dram__bytes_write.sum per launch of the two E-step kernels, from the committed ncu capture
-        tj = json.load(open(os.path.join(ROOT, "profiles", "r2_traffic.json")))
-        if world == 1 and n == 100000:
-            traffic = sum(k["dram_read_bytes"] + k["dram_write_bytes"] for k in tj["kernels"].values())
-            traffic_src = tj["source"]
-    except Exception:
-        pass
     roofline = {
         "bound": "fp32",
         "kernel": "pass1_kernel + pass2_kernel (fused E-step, never materialises P)",
@@ -513,8 +474,6 @@ def run_ours(args):
         "flop_per_pair": FLOP_PER_PAIR_ITER, "pairs_per_launch": float(n_local) * float(n),
         "instruction_ceiling_frac": ach_tf / (probe["ffma_tflops"] * (29.0 / (19.0 * 2.0))),
         "mufu_ex2_gops_probe": probe["mufu_ex2_gops"],
-        "traffic": traffic,
-        "traffic_source": traffic_src,
         "hbm": {"bound": "hbm", "achieved": bytes_iter / (t_estep_ms * 1e-3) / 1e9, "peak": hbm_peak, "unit": "GB/s",
                 "frac": bytes_iter / (t_estep_ms * 1e-3) / 1e9 / hbm_peak, "peak_source": hbm_src,
                 "algorithmic_bytes": bytes_iter,
@@ -527,7 +486,7 @@ def run_ours(args):
     out = {
         "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3),
         "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
-        "dtype": "f32", "dtype_note": "pair arithmetic f32 (packed f32x2); every sum beyond 64 terms, the moments and the M-step f64",
+        "dtype": "f32", "dtype_note": "pair arithmetic f32; every sum beyond 64 terms, the moments and the M-step f64",
         "data": "synthetic",
         "config": {"workload": workload_string(args.config, n), "baseline_config": args.config, "also": also,
                    "sharded_equals_single_gpu": (shard_check or {}).get("agree"),
@@ -559,7 +518,7 @@ def run_ours(args):
 
 def run_also(args):
     """Short runs of BASELINE configurations 3 and 5 in SUBPROCESSES (a fault there costs the main line nothing but this key);
-    the compact summaries travel inside `config`, which the driver's record keeps."""
+    the compact summaries travel inside `config` of the bench line."""
     out = {}
     for cfg, steps in ((3, 5), (5, 10)):
         try:
@@ -579,28 +538,29 @@ def run_also(args):
     return out
 
 
-def gram_roofline(n, ms_four_products):
-    """Tensor roofline of the G X product kernel (gi_gram_ts_kernel): 6 int8 MMAs of 128 x 112 x 32 per 32 points, row tile and column
-    pass (2 passes for K = 200) against the int8 rate = twice the measured bf16 peak (MEASURED_PEAKS.json, burst)."""
+def gram_roofline(n, ms_four_products, K=200):
+    """Tensor roofline of the G X product kernel (gi_gram_kernel): 6 int8 MMAs of 128 x 64 x 32 per 32 points, row tile and column
+    pass (4 passes of 64 columns for K = 200) against the int8 rate = twice the bf16 peak (MEASURED_PEAKS.json, else the data sheet)."""
     if not ms_four_products or ms_four_products <= 0:
         return None
     try:
         bf16 = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["bf16_tflops"])
         src = "2 x measured bf16 (MEASURED_PEAKS.json)"
     except Exception:
-        bf16, src = 1590.0, "2 x fallback bf16 (B200_PROFILING.md)"
+        bf16, src = 989.0, "2 x dense bf16 of the H100 SXM data sheet"
     tiles = (n + 127) // 128
     stages = ((n + 511) // 512 * 512) // 32
-    ops = 4 * 2 * tiles * stages * 6 * 2.0 * 128 * 112 * 32            # 4 products x 2 column passes
+    passes = (K + 63) // 64
+    ops = 4 * passes * tiles * stages * 6 * 2.0 * 128 * 64 * 32            # 4 products x the column passes
     ach = ops / (ms_four_products * 1e-3) / 1e12
-    return {"bound": "tensor", "kernel": "gi_gram_ts_kernel (+ split / reduce / column maxima inside the timed phase)", "achieved": ach,
+    return {"bound": "tensor", "kernel": "gi_gram_kernel (+ split / reduce / column maxima inside the timed phase)", "achieved": ach,
             "peak": 2.0 * bf16, "unit": "Top/s (int8)", "frac": ach / (2.0 * bf16), "peak_source": src}
 
 
 def run_nonrigid(args, torch, _cabi, cpd, barrier, local_rank, world):
     """BASELINE configuration 5: non-rigid CPD with G ~= Q Bc Q^T of rank 200 (no reference counterpart: the reference solves the
     dense M x M system, cpd.py:296).  A step = one EM iteration (E-step + low-rank M-step, cpd_nonrigid_step); the one-off
-    factorisation (range finder on tcgen05 G X products + blocked orthonormalisation) is reported as `setup_ms`."""
+    factorisation (range finder on tensor-core G X products + blocked orthonormalisation) is reported as `setup_ms`."""
     rank = int(os.environ.get("RANK", "0"))
     n, K = args.points, 200
     src, tgt = workload(n, "nonrigid")
@@ -646,6 +606,8 @@ def run_nonrigid(args, torch, _cabi, cpd, barrier, local_rank, world):
     clocks = sampler.stop(t_wall0, t_wall1, t_up) if sampler else None
     per_step = np.array([h.event_elapsed(2 * i, 2 * i + 1) for i in range(args.steps)])
     ms_per_step = float(per_step.sum()) / args.steps
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"sigma2": sig, "w": h.nonrigid_w(), "moved": h.nonrigid_moved()})
     h.set_profiling(True)
     stages = []
     for _ in range(5):
@@ -679,15 +641,15 @@ def run_nonrigid(args, torch, _cabi, cpd, barrier, local_rank, world):
     out = {
         "metric": METRIC, "value": 1e3 / ms_per_step, "unit": UNIT, "n_gpus": 1, "steps": args.steps, "warmup": max(args.warmup, 3),
         "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "f32",
-        "dtype_note": "pair arithmetic f32; G X products TF32 x3 (hi/lo split) on tcgen05 with FP32 TMEM accumulation per 2048-point chunk, "
-                      "FP64 across chunks; factors, K x K system and its LU f64",
+        "dtype_note": "pair arithmetic f32; G X products on 8-bit integer digits (wgmma, exact int32 accumulation per chunk of <= 16384 "
+                      "points, FP64 across chunks); factors and the K x K system f64",
         "data": "synthetic",
         "config": {"workload": workload_string(args.config, n), "baseline_config": args.config,
                    "parallelism": "single GPU", "l2": "flushed (256 MiB memset) between timed iterations, outside the event pairs",
                    "timing": "CUDA event pair per iteration on the library stream, summed"},
         "setup_ms": setup_wall_ms, "setup_cold_ms": setup_cold_ms,
-        "setup": dict(setup, what="one-off per source: 4 products G X (K = 200: tcgen05 kind::i8, 8-bit digit planes, A operand and int32 "
-                                  "accumulators in TMEM) + 3 blocked orthonormalisations + Q^T G Q",
+        "setup": dict(setup, what="one-off per source: 4 products G X (K = 200: wgmma on 8-bit digit planes, A operand generated into "
+                                  "registers, int32 accumulators) + 3 blocked orthonormalisations + Q^T G Q",
                       gram_tflops_useful=(4 * gram_flop / (setup["gram_products_ms"] * 1e-3) / 1e12) if setup["gram_products_ms"] > 0 else None,
                       gram_roofline=gram_roofline(n, setup["gram_products_ms"])),
         "e2e": {"value": 1.0 / e2e_s, "unit": UNIT, "h2d_bytes_per_step": int(src.nbytes + tgt.nbytes), "d2h_bytes_per_step": int(8 + src.nbytes),
@@ -725,6 +687,28 @@ def run_extras():
         return {"error": "%s: %s" % (type(e).__name__, str(e)[:300])}
 
 
+DUMP_ROWS = 500000
+
+
+def dump_outputs(d, arrays):
+    """DIR/<name>.npy, float64, for every array (or scalar) of `arrays`.  Arrays of more than DUMP_ROWS rows: a sample of
+    DUMP_ROWS rows drawn with a seed that depends only on the row count (the same rows in every run and build), the sorted row
+    indices in DIR/<name>_rows.npy.  At most three such arrays of up to 3 columns: < 32 MB in all."""
+    os.makedirs(d, exist_ok=True)
+    total = 0
+    for name, a in arrays.items():
+        a = np.asarray(a, dtype=np.float64)
+        if a.ndim >= 1 and a.shape[0] > DUMP_ROWS:
+            rows = np.sort(np.random.default_rng(a.shape[0]).choice(a.shape[0], DUMP_ROWS, replace=False))
+            a = a[rows]
+            np.save(os.path.join(d, name + "_rows.npy"), rows.astype(np.float64))
+            total += rows.nbytes
+        np.save(os.path.join(d, name + ".npy"), a)
+        total += a.nbytes
+    if total > 64 << 20:
+        raise SystemExit("--dump-outputs: %d bytes, more than 64 MB" % total)
+
+
 def emit(obj):
     """The ONE JSON line goes to the real stdout; everything else this process (or NCCL, which
     prints its version banner to fd 1) writes during the run has been diverted to stderr."""
@@ -748,6 +732,8 @@ def main():
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
     ap.add_argument("--no-also", action="store_true", help="skip the short runs of configurations 3 and 5 reported under config.also")
     ap.add_argument("--extras", action="store_true", help="add the side measurements of tools/bench_extras.py (key \"extras\")")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the timed path computed in its last step to DIR/<name>.npy (float64)")
     args = ap.parse_args()
     args.kind = WORKLOADS[args.config][0]
     if args.points <= 0:

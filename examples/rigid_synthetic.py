@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Rigid CPD of two 100k-point clouds on one B200 (the reference's examples/cpd_rigid_cuda.py, without open3d)."""
+"""Rigid CPD of two 100k-point clouds on one H100 (the reference's examples/cpd_rigid_cuda.py, without open3d)."""
 import os
 import sys
 import time

@@ -48,8 +48,9 @@ def prepare_source_and_target_nonrigid_3d(source_filename, target_filename, voxe
 
 def reference_file(name):
     """Path of one of the reference's example data files (bunny.pcd, fish_source.txt, face-x.txt, ...): next to this script, under
-    $PROBREG_EXAMPLES, or in a probreg checkout at /root/reference/examples; None when it is nowhere."""
-    for d in (os.path.dirname(os.path.abspath(__file__)), os.environ.get("PROBREG_EXAMPLES", ""), "/root/reference/examples"):
+    $PROBREG_EXAMPLES, or among the copies kept for the tests (tests/golden/data); None when it is nowhere."""
+    here = os.path.dirname(os.path.abspath(__file__))
+    for d in (here, os.environ.get("PROBREG_EXAMPLES", ""), os.path.join(os.path.dirname(here), "tests", "golden", "data")):
         if d and os.path.exists(os.path.join(d, name)):
             return os.path.join(d, name)
     return None

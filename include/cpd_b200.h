@@ -1,5 +1,5 @@
 /*
- * cpd_b200.h -- C ABI of libcpd_b200.so: the CPD EM hot path on one B200 (sm_100a).
+ * cpd_b200.h -- C ABI of libcpd_b200.so: the CPD EM hot path on one H100 (sm_90a).
  *
  * The reference (neka-nat/probreg v0.3.7) has no C/FFI boundary for this path: the seam
  * is Python-level (probreg/cpd.py) plus one pybind11 module (probreg/_math).  Each entry

@@ -7,8 +7,8 @@ the checker or the CPU arm being timed.  Nothing under ``probreg_b200/`` imports
 the product path has no CPU fallback.
 
 Parity status: PINNED.  ``tests/golden/make_golden.py`` imports the reference's own
-``probreg/cpd.py`` unmodified (in the build container, where ``/root/reference``
-exists) and stores its outputs in ``tests/golden/*.npz``; ``tests/test_oracle.py``
+``probreg/cpd.py`` unmodified (from a reference checkout named by $PROBREG_REFERENCE)
+and stores its outputs in ``tests/golden/*.npz``; ``tests/test_oracle.py``
 checks every function below against those fixtures.
 
 Reference lines restated here (all paths relative to the reference repo):
@@ -105,7 +105,7 @@ def sigma2_init(source, target, max_dense=int(4e7)):
 
 
 def sigma2_init_exact(source, target):
-    """Closed form of the same quantity in float64 (SURVEY appendix A.4)."""
+    """Closed form of the same quantity in float64."""
     m, d = source.shape
     n = target.shape[0]
     sx = np.sum(target * target)

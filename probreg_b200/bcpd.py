@@ -1,7 +1,7 @@
-"""Bayesian Coherent Point Drift -- the API surface of ``probreg.bcpd`` with the E-step on the B200.
+"""Bayesian Coherent Point Drift -- the API surface of ``probreg.bcpd`` with the E-step on the H100.
 
-SURVEY section 8(f) row 3.  What is accelerated is ``BayesianCoherentPointDrift.expectation_step`` (reference: bcpd.py:53-72): it is
-the CPD E-step with one weight per source point and runs in the same two sm_100a passes (``cpd_bcpd_estep``, the ``WGT``
+What is accelerated is ``BayesianCoherentPointDrift.expectation_step`` (reference: bcpd.py:53-72): it is
+the CPD E-step with one weight per source point and runs in the same two sm_90a passes (``cpd_bcpd_estep``, the ``WGT``
 instantiations of the pair kernels), so the M x N matrix the reference materialises never exists.  The M-step of ``CombinedBCPD``
 (reference: bcpd.py:127-156) is dense M x M linear algebra that the reference itself performs on the host -- two matrix inverses per
 iteration -- and is outside the accelerated path; it is restated below, split into the three things it computes, so that

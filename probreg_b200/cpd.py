@@ -2,7 +2,7 @@
 
 Drop-in for probreg/cpd.py: ``registration_cpd``, ``RigidCPD``, ``AffineCPD``, ``NonRigidCPD``, ``ConstrainedNonRigidCPD``,
 ``EstepResult``, ``MstepResult`` keep their names, arguments, return types and error behaviour.
-What differs is where the work happens: every E-step / M-step runs in hand-written sm_100a
+What differs is where the work happens: every E-step / M-step runs in hand-written sm_90a
 kernels behind the C ABI of ``libcpd_b200.so`` (include/cpd_b200.h).  There is no numpy path
 and no CPU fallback; ``use_cuda`` is accepted for signature compatibility and ignored (the
 reference's False default would select its numpy path, which does not exist here).
@@ -47,7 +47,7 @@ class CoherentPointDrift(abc.ABC):
     """EM driver (probreg/cpd.py:28-120).  The E-step is implemented here, the M-step in the
     subclasses -- both as calls into the CUDA library.
 
-    ``source``: (M, D) array or None; ``use_cuda``: ignored, the sm_100a kernels are the only implementation;
+    ``source``: (M, D) array or None; ``use_cuda``: ignored, the sm_90a kernels are the only implementation;
     ``device``: CUDA ordinal (default: the communicator's, else 0); ``comm``: a probreg_b200.dist.Communicator
     for multi-GPU target sharding.
     """
@@ -249,7 +249,7 @@ class AffineCPD(CoherentPointDrift):
 class NonRigidCPD(CoherentPointDrift):
     """Coherent Point Drift for nonrigid transformation (probreg/cpd.py:247-303).
 
-    SURVEY section 8(f) row 1: ``registration`` keeps G (float32, like ``_math.rbf_kernel``), W and the
+    ``registration`` keeps G (float32, like ``_math.rbf_kernel``), W and the
     M x M system on the device -- E-step by the CPD kernels, the dense solve of cpd.py:296 by cuSOLVER's LU,
     sigma2 in residual form.  ``maximization_step`` on a caller-supplied EstepResult runs the same solve on the
     device (cpd_nonrigid_mstep) with sigma2 from the reference's three traces.
@@ -485,7 +485,7 @@ def registration_cpd(source, target, tf_type_name="rigid", w=0.0, maxiter=50, to
     w              -- weight of the uniform outlier component, 0 <= w < 1
     maxiter, tol   -- at most maxiter EM iterations; stop once |q - q_prev| < tol
     callbacks      -- callables invoked as cb(transformation) after every iteration
-    use_cuda       -- accepted for compatibility, ignored: the B200 kernels are the only implementation
+    use_cuda       -- accepted for compatibility, ignored: the H100 kernels are the only implementation
     **kwargs       -- forwarded to the class: update_scale, tf_init_params, beta, lmd, alpha, idx_source,
                       idx_target, and the extensions device= / comm=
     Returns MstepResult(transformation, sigma2, q).

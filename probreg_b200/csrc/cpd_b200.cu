@@ -4,7 +4,6 @@
 #include "cpd_b200.h"
 #include "kernels.cuh"
 #include "lowrank.cuh"
-#include "gram_umma.cuh"
 #include "gram_i8.cuh"
 
 #include <cub/device/device_radix_sort.cuh>
@@ -154,7 +153,7 @@ constexpr int CUDA_R_64F_ = 1, CUBLAS_OP_T_ = 1;
 // handle
 // ---------------------------------------------------------------------------------------------
 struct cpd_ctx {
-    int device = 0, dim = 3, sm_count = 148, slots1 = 296, slots2 = 296;
+    int device = 0, dim = 3, sm_count = 132, slots1 = 264, slots2 = 264;
     cudaStream_t stream = nullptr;
     bool own_stream = false;
     long long m = 0, mpad = 0, n = 0, npad = 0, n_global = 0;
@@ -224,12 +223,9 @@ struct cpd_ctx {
            *d_lr_R = nullptr, *d_lr_sys = nullptr, *d_lr_rhs = nullptr, *d_lr_c = nullptr, *d_lr_out = nullptr, *d_lr_panel = nullptr, *d_lr_Lt = nullptr;
     bool lr_spd = true;                   // symmetric positive definite K x K system on Qt = Q L (lr_spd_form); CPD_B200_LR_CORE=lu: LU of (c I + Bc S)
     size_t lr_part_cap = 0;               // doubles in d_lr_part (slice partials of lr_inner)
-    float *d_gu_planes = nullptr, *d_gu_part = nullptr;      // tcgen05 G X product: TF32 hi / lo planes of X, chunk partials
-    size_t gu_planes_cap = 0, gu_part_cap = 0;
     unsigned char* d_gi_planes = nullptr;                      // exact int8-digit product: digit planes of X, FP64 chunk partials, column maxima
     double *d_gi_part = nullptr, *d_gi_colmax = nullptr;
-    size_t gi_planes_cap = 0, gi_part_cap = 0, gi_colmax_cap = 0, gi_pairs_cap = 0;
-    float4* d_gi_pairs = nullptr;                            // the scaled source points as packed pair records (generators' f32x2 maths)
+    size_t gi_planes_cap = 0, gi_part_cap = 0, gi_colmax_cap = 0;
     size_t lr_out_cap = 0;
     P2PMailbox* d_box = nullptr;          // this rank's mailbox (peers write into it)
     P2PInfo* d_p2p = nullptr;             // device copy of the peer table; non-null => fused P2P exchange
@@ -272,8 +268,8 @@ inline unsigned blocks_for(long long n) { return (unsigned)((n + THREADS - 1) / 
 // Work list of one pass: every i-tile is cut into J contiguous stage ranges ("splits"), one CTA each; J is chosen to
 // minimise the makespan  ceil(ntiles*J / slots) * (ceil(nstages/J) + pipeline fill)  over the resident CTA slots, and slots
 // left over in a single-wave launch go to extra splits of the first tiles.  All tiles carry the same work, so this is within
-// one stage of the optimum whatever N, M and the GPU count are.  (A finer "stream-K" cut that lets one CTA span two tiles was
-// measured 15-19 % slower: the extra live state pushes the hot loops past 128 registers.)
+// one stage of the optimum whatever N, M and the GPU count are.  (A finer "stream-K" cut that lets one CTA span two tiles needs
+// extra live state in the hot loops, which already sit at the 128-register cap.)
 struct WorkList {
     std::vector<int4> items;        // {tile, first unit, end unit, slot within the tile}; a unit is a sub-chunk of SUB j-records
     std::vector<int> tile_slots;    // partial slots used per tile
@@ -457,12 +453,10 @@ int prepare(cpd_ctx* h) {
     if (!h->have_source || !h->have_target) return fail(CPD_ERR_STATE, "source and target must both be set");
     h->it1 = (int)((h->n + ITILE1 - 1) / ITILE1);
     h->it2 = (int)((h->m + ITILE2 - 1) / ITILE2);
-    // Pass 1 cuts at sub-chunks, and the warps of its last i-tile whose i-points are all padding leave the kernel at once.  What such
-    // a tile then costs was measured (1/8 and 1/4 target shards of 100k: 2 and 4 of 8 warps alive; profiles/r2_plan_sweep.txt): the
-    // best plans come from a cost of 0.6 of a full tile in BOTH cases -- not w / 8: the live warps get a larger share of the SM's
-    // pipes, but a warp on its own is latency-bound (0.45 makes the tile's few long items set the time: +10 %; 1.0 wastes the early
-    // exit: +2..4 %).  Pass 2 keeps whole stages as the unit (its kernel is the one closest to the register limit; cutting it at
-    // sub-chunks cost 1.4 % at every size).
+    // Pass 1 cuts at sub-chunks, and the warps of its last i-tile whose i-points are all padding leave the kernel at once.  Such a
+    // tile is planned at max(0.6, live warps / 8) of a full tile, not live / 8: the live warps get a larger share of the SM's pipes,
+    // but a warp on its own is latency-bound.  Pass 2 keeps whole stages as the unit (its kernel is the one closest to the register
+    // limit).  The 0.6 and the units are not tuned for the H100; CPD_B200_PLAN_LAST_COST and CPD_B200_PLAN_UNIT switch them.
     const long long in_last = h->n - (long long)(h->it1 - 1) * ITILE1;
     const int live = (int)((in_last + 32 * RI1 - 1) / (32 * RI1));          // warps of the last tile that hold i-points
     double last_cost = live < THREADS / 32 ? std::max(0.6, live / (double)(THREADS / 32)) : 1.0;
@@ -618,7 +612,8 @@ extern "C" int cpd_create(cpd_ctx** out, int device, int dim, void* stream) {
     CU(cudaSetDevice(device));
     cudaDeviceProp prop;
     CU(cudaGetDeviceProperties(&prop, device));
-    if (prop.major < 10) return fail(CPD_ERR_CUDA, "device %d is sm_%d%d; this library is built for sm_100a only", device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0)
+        return fail(CPD_ERR_CUDA, "device %d is sm_%d%d; this library is built for sm_90a (Hopper) only", device, prop.major, prop.minor);
     cpd_ctx* h = new cpd_ctx();
     h->device = device;
     h->dim = dim;
@@ -670,7 +665,7 @@ extern "C" void cpd_destroy(cpd_ctx* h) {
     void* nrp[] = {h->d_G, h->d_W, h->d_A, h->d_B, h->d_ts2, h->d_nrpart, h->d_ipiv, h->d_info, h->d_work};
     for (void* p : nrp) if (p) cudaFree(p);
     void* lrp[] = {h->d_lr_pts, h->d_lr_Q, h->d_lr_X, h->d_lr_coef, h->d_lr_part, h->d_lr_Bc, h->d_lr_S, h->d_lr_R, h->d_lr_sys, h->d_lr_rhs,
-                   h->d_lr_c, h->d_lr_out, h->d_lr_panel, h->d_lr_Lt, h->d_gu_planes, h->d_gu_part, h->d_gi_planes, h->d_gi_part, h->d_gi_colmax, h->d_gi_pairs, h->d_wgt, h->d_p1t, h->d_pxt, h->d_la, h->d_log2c};
+                   h->d_lr_c, h->d_lr_out, h->d_lr_panel, h->d_lr_Lt, h->d_gi_planes, h->d_gi_part, h->d_gi_colmax, h->d_wgt, h->d_p1t, h->d_pxt, h->d_la, h->d_log2c};
     for (void* p : lrp) if (p) cudaFree(p);
     if (h->h_work) free(h->h_work);
     if (h->sol_params && g_sol.DestroyParams) g_sol.DestroyParams(h->sol_params);

@@ -1,11 +1,9 @@
 // gram_i8.cuh -- the Gram-matrix product  out[c][i] = sum_j G_ij X[c][j]  with EXACT accumulation on the tensor cores:
-// both operands are cut into 8-bit digits and multiplied with tcgen05.mma kind::i8 (unsigned x signed, 32-bit integer
-// accumulators in TMEM).  Integer MMAs do not round, so -- unlike the TF32 x 3 kernel of gram_umma.cuh, whose FP32 TMEM
-// accumulation truncates once per MMA (measured: a systematic shrink of ~1e-5 over a 2048-point chunk, profiles/r2_umma_*) --
-// the only errors are the two quantisations (2^-24 absolute on G, 2^-23 of the column maximum on X), at the level of the float32 G
-// the reference itself uses
-// (cc/math_utils.cc:17-19).  Same role as gram_umma.cuh: the products of the low-rank range finder (probreg/cpd.py:296-297 with
-// G = rbf_kernel(Y, Y, beta) of transformation.py:91-102, never stored).
+// both operands are cut into 8-bit digits and multiplied with Hopper's warpgroup MMA (wgmma.mma_async m64n64k32, unsigned x
+// signed 8-bit, 32-bit integer accumulators in registers).  Integer MMAs do not round, so the only errors are the two
+// quantisations (2^-24 absolute on G, 2^-23 of the column maximum on X), at the level of the float32 G the reference itself uses
+// (cc/math_utils.cc:17-19).  Role: the products of the low-rank range finder (probreg/cpd.py:296-297 with
+// G = rbf_kernel(Y, Y, beta) of transformation.py:91-102); G is never stored -- it is generated tile by tile on the CUDA cores.
 //
 // Fixed point ("Ozaki splitting" with integer digits):
 //     g_ij = round(2^23 G_ij) in [0, 2^23]         = a0 2^16 + a1 2^8 + a2,     a_s in [0, 255]        (unsigned digits, a0 <= 128)
@@ -15,61 +13,66 @@
 // An accumulator receives at most 3 products of magnitude < 2^15 per point: exact in int32 for chunks of up to 16384 points.
 // The epilogue joins the three levels in FP64 (exact) and applies the column scale; chunk partials are added in a fixed order.
 //
-// Two kernels: gi_gram_kernel (A operand in shared memory) and gi_gram_ts_kernel (A operand in tensor memory: the default, see below).
-// CTA = 128 rows of G x up to 112 columns (3 accumulators x 112 columns of TMEM); the columns of X are taken in passes of <= 112,
-// G is regenerated per pass (the generator needs ~2/3 of the MMA time).  Persistent over {row tile, column pass, j-chunk};
-// warp roles, pipeline and barriers as in gram_umma.cuh, with 32-point stages (one MMA K-step) and 8 stages of 24 KB.
-// Shared-memory operand layout: K-major, 32-byte rows, SWIZZLE_32B: row r at byte 32 r (8-row groups 256 B apart), the 16-byte
-// half h of a row at position h ^ ((r >> 2) & 1).
-// The digit planes of X are stored in global memory AS the shared-memory image of each stage (gi_split_kernel: point block jb ->
-// 3 planes x 4096 bytes, rows already swizzled), so a stage's B operand is ONE 12 KB bulk copy (cp.async.bulk, SASS UBLKCP).
-// A tensor-map box of 32-byte rows -- the first version of this kernel, and the 64-byte rows of gram_umma.cuh -- is limited by the
-// TMA unit's row rate, measured at ~4.5 cycles per box row per SM: 336 rows = 1470 cycles per stage against 360 cycles of MMAs.
+// CTA = GI_WG consumer warpgroups of 64 rows each + one producer warp, persistent over work units {row tile, j-chunk}; the
+// columns of X are taken in passes of GI_N = 64 (3 levels x 32 accumulator registers per thread).
+//     producer warp   one lane streams each 32-point stage -- the three digit planes of X (the B operands, 3 x 2 KB) and the
+//                     stage's 32 j-points (512 B) -- into a ring of GI_STAGES shared-memory slots with bulk copies (TMA,
+//                     cp.async.bulk) completing on the slot's `full` mbarrier
+//     warpgroups      generate their 64 x 32 tile of G straight into the wgmma A-operand register fragment (no shared-memory
+//                     round trip for A), issue the six MMAs, wait for them and release the slot (`empty` mbarrier, one arrival
+//                     per warp).  While one warpgroup waits on its MMAs the others generate: the CUDA-core work and the
+//                     tensor-core work of the SM overlap across warpgroups.
+// Shared-memory B layout: K-major, 32-byte rows, 32-byte swizzle: row r at byte 32 r (8-row groups 256 B apart = the descriptor's
+// stride byte offset), the 16-byte half h of a row at position h ^ ((r >> 2) & 1).  gi_split_kernel stores the digit planes of X in
+// global memory AS these stage images, so a stage is one bulk copy.
 #pragma once
 #ifndef CPD_HOST_EMU
-#include "gram_umma.cuh"
+#include "kernels.cuh"
 
 namespace cpd {
 
-constexpr int GI_ROWS = 128;
-constexpr int GI_KS = 32;              // j-points per stage = one kind::i8 MMA K-step (32 bytes per row)
-constexpr int GI_NMAX = 112;           // columns per pass (3 levels x 112 = 336 TMEM columns)
+constexpr int GI_WG = 2;                               // consumer warpgroups per CTA
+constexpr int GI_ROWS = 64 * GI_WG;                    // rows of G per work unit
+constexpr int GI_KS = 32;                              // j-points per stage = one m64n64k32 K-step (32 bytes per row)
+constexpr int GI_N = 64;                               // columns of X per pass (the MMA's N)
 constexpr int GI_STAGES = 8;
-constexpr int GI_PLANE = 4096;         // bytes reserved per digit plane of a stage (128 x 32 used for A, n16 x 32 for B)
-constexpr int GI_STAGE_BYTES = 6 * GI_PLANE;
-constexpr int GI_THREADS = 14 * 32;
-constexpr int GI_PTS_BYTES = GI_KS * 16;                  // the stage's 32 j-points (float4), staged by the same TMA producer
-constexpr int GI_SMEM = GI_STAGES * (GI_STAGE_BYTES + GI_PTS_BYTES) + 1024 + 256;
+constexpr int GI_PLANE = GI_N * GI_KS;                 // bytes of one digit plane of a stage (2 KB)
+constexpr int GI_PTS_BYTES = GI_KS * 16;               // the stage's 32 j-points (float4)
+constexpr int GI_THREADS = GI_WG * 128 + 32;
+constexpr int GI_SMEM = GI_STAGES * (3 * GI_PLANE + GI_PTS_BYTES) + 256 /* alignment slack */ + 256 /* barriers */;
 constexpr int GI_MAX_CHUNK = 16384;
 
-__device__ __forceinline__ void gi_mma_i8(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+// ---- PTX wrappers ---------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void gi_mbar_arrive(uint64_t* bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+// shared-memory matrix descriptor of a K-major operand with 32-byte swizzle: start >> 4 in [0,14), leading byte offset >> 4 in
+// [16,30) (unused for a swizzled K-major operand whose K extent is one swizzle row; 1 by convention), stride byte offset >> 4 in
+// [32,46) (8 rows x 32 B = 256), layout type in [62,64): 3 = 32-byte swizzle
+__device__ __forceinline__ uint64_t gi_smem_desc(uint32_t saddr) {
+    return (uint64_t)((saddr & 0x3ffffu) >> 4) | (1ull << 16) | ((uint64_t)(256 >> 4) << 32) | (3ull << 62);
+}
+__device__ __forceinline__ uint32_t gi_row_half_offset(int r, int h) { return (uint32_t)(r * 32 + ((h ^ ((r >> 2) & 1)) << 4)); }
+__device__ __forceinline__ void gi_wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void gi_wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void gi_wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// D[64 x 64] (+)= A[64 x 32] (u8, this thread's register fragment) * B[32 x 64] (s8, K-major in shared memory)
+__device__ __forceinline__ void gi_mma(int (&d)[32], const uint32_t (&a)[4], uint64_t bdesc, int accumulate) {
     asm volatile(
         "{\n"
         ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n"
-        "}" ::"r"(d_tmem),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
+        "setp.ne.b32 p, %37, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k32.s32.u8.s8 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "{%32, %33, %34, %35}, %36, p;\n"
+        "}"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]),
+          "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]),
+          "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]),
+          "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate)
         : "memory");
-}
-// K-major, SWIZZLE_32B (layout type 6), 8-row groups 256 bytes apart
-__device__ __forceinline__ uint64_t gi_smem_desc(uint32_t saddr) {
-    return (uint64_t)((saddr & 0x3ffffu) >> 4) | (1ull << 16) | ((uint64_t)(256 >> 4) << 32) | (1ull << 46) | (6ull << 61);
-}
-// D = S32 (2 at [4,6)), A = unsigned 8-bit (0 at [7,10)), B = signed 8-bit (1 at [10,13)), K-major, N >> 3 at [17,23), M >> 4 at [24,29)
-__host__ __device__ __forceinline__ uint32_t gi_instr_desc(int n) {
-    return (2u << 4) | (0u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-}
-__device__ __forceinline__ uint32_t gi_row_half_offset(int r, int h) { return (uint32_t)(r * 32 + ((h ^ ((r >> 2) & 1)) << 4)); }
-__device__ __forceinline__ void gi_tmem_ld16(uint32_t taddr, int (&v)[16]) {
-    uint32_t r[16];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-                   "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                 : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int k = 0; k < 16; ++k) v[k] = (int)r[k];
 }
 
 // ---- operand preparation -----------------------------------------------------------------------------------------------------------
@@ -134,35 +137,40 @@ gi_reduce_kernel(const double* __restrict__ part, int nq, int n16, long long ldp
         out[(long long)c * ld + i_begin + ii] = s;
     }
 }
-
-// j-points as packed pairs for the generators' f32x2 arithmetic: record k (32 bytes) = {x_2k, x_2k+1, y_2k, y_2k+1}, {z_2k, z_2k+1, 0, 0}
+// first-use self-check: the largest |a - b| and |b| over rows [0, rows) of `cols` columns  ->  res[0], res[1] (one CTA)
 __global__ void __launch_bounds__(THREADS)
-gi_pairs_kernel(const float4* __restrict__ pts, long long npairs, float4* __restrict__ rec) {
-    const long long k = (long long)blockIdx.x * THREADS + threadIdx.x;
-    if (k < npairs) {
-        const float4 p = pts[2 * k], q = pts[2 * k + 1];
-        rec[2 * k] = make_float4(p.x, q.x, p.y, q.y);
-        rec[2 * k + 1] = make_float4(p.z, q.z, 0.0f, 0.0f);
+gi_compare_kernel(const double* __restrict__ a, const double* __restrict__ b, long long ld, long long i_begin, long long rows, int cols,
+                  double* __restrict__ res) {
+    __shared__ double sd[THREADS], sv[THREADS];
+    double d = 0.0, v = 0.0;
+    for (int c = 0; c < cols; ++c)
+        for (long long i = threadIdx.x; i < rows; i += THREADS) {
+            const double x = a[(long long)c * ld + i_begin + i], y = b[(long long)c * ld + i_begin + i];
+            d = fmax(d, fabs(x - y)); v = fmax(v, fabs(y));
+            if (!(x == x)) d = 1e300;                      // NaN in the tensor-core result
+        }
+    sd[threadIdx.x] = d; sv[threadIdx.x] = v;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int t = 1; t < THREADS; ++t) { d = fmax(d, sd[t]); v = fmax(v, sv[t]); }
+        res[0] = d; res[1] = v;
     }
 }
 
 // ---- the product -----------------------------------------------------------------------------------------------------------------
-// one column pass: images = the stage images of gi_split_kernel (jpad / 32 of them); rows [i_begin, i_end) of G;
-// part[q][c][ii] (FP64) = colmax[c] 2^-45 sum_{j in chunk q} g_ij x_cj
+// one column pass: images = the stage images of gi_split_kernel (jpad / 32 of them); pts: float4 {a, 0} per point in the scaled frame
+// of lr_pack_kernel, padded to jpad with far-away records (G == 0); rows [i_begin, i_end) of G;
+// part[q][c][ii] (FP64) = colmax[c] 2^-45 sum_{j in chunk q} g_ij x_cj  for c < GI_N, ii < ldp (a multiple of GI_ROWS)
 __global__ void __launch_bounds__(GI_THREADS, 1)
-gi_gram_kernel(const unsigned char* __restrict__ images, const float4* __restrict__ pts, const float4* __restrict__ pairs, long long jpad, int chunk,
-               long long i_begin,
-               long long i_end, int n16, const double* __restrict__ colmax, double* __restrict__ part, long long ldp) {
-    extern __shared__ __align__(1024) unsigned char gu_smem_raw[];
-    unsigned char* smem = gu_smem_raw;
-    unsigned char* spts = smem + GI_STAGES * GI_STAGE_BYTES;            // [GI_STAGES][32] float4: the j-points of each stage
-    uint64_t* bars = reinterpret_cast<uint64_t*>(spts + GI_STAGES * GI_PTS_BYTES);
-    uint64_t* full_a = bars;
-    uint64_t* full_b = bars + GI_STAGES;
-    uint64_t* empty = bars + 2 * GI_STAGES;
-    uint64_t* acc_full = bars + 3 * GI_STAGES;
-    uint64_t* acc_empty = bars + 3 * GI_STAGES + 1;
-    uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(bars + 3 * GI_STAGES + 2);
+gi_gram_kernel(const unsigned char* __restrict__ images, const float4* __restrict__ pts, long long jpad, int chunk, long long i_begin,
+               long long i_end, const double* __restrict__ colmax, double* __restrict__ part, long long ldp) {
+    // 256-byte alignment anchors the 32-byte swizzle pattern of every B plane the way the MMA unit reads it
+    extern __shared__ __align__(256) unsigned char gi_smem_raw[];
+    unsigned char* planes = gi_smem_raw;                                      // [GI_STAGES][3][GI_PLANE]
+    const float4* spts = reinterpret_cast<const float4*>(planes + GI_STAGES * 3 * GI_PLANE);     // [GI_STAGES][GI_KS]
+    uint64_t* bars = reinterpret_cast<uint64_t*>(planes + GI_STAGES * (3 * GI_PLANE + GI_PTS_BYTES));
+    uint64_t* full = bars;                     // [GI_STAGES]: the slot's bytes have landed
+    uint64_t* empty = bars + GI_STAGES;        // [GI_STAGES]: every warp of every warpgroup is done with the slot
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const long long rows = i_end - i_begin;
@@ -171,19 +179,13 @@ gi_gram_kernel(const unsigned char* __restrict__ images, const float4* __restric
     const long long nunits = (long long)ntiles * nq;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < GI_STAGES; ++s) { mbar_init(&full_a[s], 8); mbar_init(&full_b[s], 1); mbar_init(&empty[s], 1); }
-        mbar_init(acc_full, 1);
-        mbar_init(acc_empty, 4);
+        for (int s = 0; s < GI_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 4 * GI_WG); }
         mbar_fence_init();
     }
-    if (warp == 1) gu_tmem_alloc(tmem_base_slot, 512);
-    gu_tc_fence_before();
     __syncthreads();
-    gu_tc_fence_after();
-    const uint32_t tmem_base = *tmem_base_slot;
 
-    if (warp == 0) {
-        // ===== TMA producer: the stage image (three digit planes of X for 32 points), one bulk copy =====
+    if (warp == 4 * GI_WG) {
+        // ===== producer: one bulk copy of the stage image (three digit planes of X) + one of the stage's j-points =====
         if (lane == 0) {
             uint32_t stage = 0, phase = 0;
             for (long long u = blockIdx.x; u < nunits; u += gridDim.x) {
@@ -192,438 +194,99 @@ gi_gram_kernel(const unsigned char* __restrict__ images, const float4* __restric
                 const int nst = (int)((min((long long)chunk, jpad - j0)) / GI_KS);
                 const unsigned char* src = images + (j0 / GI_KS) * (3 * GI_PLANE);
                 for (int kb = 0; kb < nst; ++kb) {
-                    gu_wait(&empty[stage], phase ^ 1, 11);
-                    mbar_expect_tx(&full_b[stage], (uint32_t)(3 * GI_PLANE + GI_PTS_BYTES));
-                    tma_load_1d(smem + stage * GI_STAGE_BYTES + 3 * GI_PLANE, src + (long long)kb * (3 * GI_PLANE), (uint32_t)(3 * GI_PLANE),
-                                &full_b[stage]);
-                    tma_load_1d(spts + stage * GI_PTS_BYTES, pairs + j0 + (long long)kb * GI_KS, (uint32_t)GI_PTS_BYTES, &full_b[stage]);
+                    mbar_wait(&empty[stage], phase ^ 1);
+                    mbar_expect_tx(&full[stage], (uint32_t)(3 * GI_PLANE + GI_PTS_BYTES));
+                    tma_load_1d(planes + stage * 3 * GI_PLANE, src + (long long)kb * (3 * GI_PLANE), (uint32_t)(3 * GI_PLANE), &full[stage]);
+                    tma_load_1d((void*)(spts + stage * GI_KS), pts + j0 + (long long)kb * GI_KS, (uint32_t)GI_PTS_BYTES, &full[stage]);
                     if (++stage == GI_STAGES) { stage = 0; phase ^= 1; }
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer: level l = s + t accumulates a_s x b_t; the whole warp walks the pipeline, one elected lane issues =====
-        {
-            const uint32_t idesc = gi_instr_desc(n16);
-            uint32_t stage = 0, phase = 0, acc_phase = 0;
-            for (long long u = blockIdx.x; u < nunits; u += gridDim.x) {
-                const int q = (int)(u / ntiles);
-                const long long j0 = (long long)q * chunk;
-                const int nst = (int)((min((long long)chunk, jpad - j0)) / GI_KS);
-                gu_wait(acc_empty, acc_phase ^ 1, 12);
-                gu_tc_fence_after();
-                for (int kb = 0; kb < nst; ++kb) {
-                    gu_wait(&full_a[stage], phase, 13);
-                    gu_wait(&full_b[stage], phase, 14);
-                    gu_tc_fence_after();
-                    const uint32_t sa = smem_u32(smem) + stage * GI_STAGE_BYTES;
-                    const uint32_t sb = sa + 3 * GI_PLANE;
-                    const uint32_t first = kb != 0 ? 1u : 0u;
-                    if (gu_elect_one()) {
-                        uint64_t a[3], b[3];
+        return;
+    }
+
+    // ===== warpgroups: G tile -> A fragment, six MMAs per stage, epilogue per work unit =====
+    // A fragment of m64k32 (8-bit): warp w of the warpgroup holds rows 16 w + lane / 4 (registers 0, 2) and + 8 (registers 1, 3);
+    // register 0 / 1 carry k = 4 (lane % 4) .. + 3, registers 2 / 3 the same k + 16, lowest k in the lowest byte.
+    // Accumulator fragment of m64n64: register 4 i + h (+ 2 for row + 8) is column 8 i + 2 (lane % 4) + h.
+    const int wg = warp >> 2;
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);             // row of the tile; the other row is r0 + 8
+    const int kq = (lane & 3) * 4;
+    uint32_t stage = 0, phase = 0;
+    for (long long u = blockIdx.x; u < nunits; u += gridDim.x) {
+        const int q = (int)(u / ntiles), t = (int)(u % ntiles);
+        const long long j0 = (long long)q * chunk;
+        const int nst = (int)((min((long long)chunk, jpad - j0)) / GI_KS);
+        float ax[2], ay[2], az[2];
 #pragma unroll
-                        for (int p = 0; p < 3; ++p) { a[p] = gi_smem_desc(sa + p * GI_PLANE); b[p] = gi_smem_desc(sb + p * GI_PLANE); }
-                        gi_mma_i8(tmem_base, a[0], b[0], idesc, first);
-                        gi_mma_i8(tmem_base + (uint32_t)n16, a[0], b[1], idesc, first);
-                        gi_mma_i8(tmem_base + (uint32_t)n16, a[1], b[0], idesc, 1u);
-                        gi_mma_i8(tmem_base + (uint32_t)(2 * n16), a[0], b[2], idesc, first);
-                        gi_mma_i8(tmem_base + (uint32_t)(2 * n16), a[1], b[1], idesc, 1u);
-                        gi_mma_i8(tmem_base + (uint32_t)(2 * n16), a[2], b[0], idesc, 1u);
-                        gu_commit(&empty[stage]);
-                        if (kb == nst - 1) gu_commit(acc_full);
-                    }
-                    __syncwarp();
-                    if (++stage == GI_STAGES) { stage = 0; phase ^= 1; }
-                }
-                acc_phase ^= 1;
-            }
-        }
-    } else if (warp < 6) {
-        // ===== epilogue: join the three levels in FP64 (exact), scale, store the chunk partial =====
-        const int quarter = warp & 3;
-        uint32_t acc_phase = 0;
-        for (long long u = blockIdx.x; u < nunits; u += gridDim.x) {
-            const int q = (int)(u / ntiles), t = (int)(u % ntiles);
-            gu_wait_relaxed(acc_full, acc_phase, 15);
-            gu_tc_fence_after();
-            const long long ii = (long long)t * GI_ROWS + quarter * 32 + lane;
-            double* dst = part + (long long)q * n16 * ldp + ii;
-            const uint32_t tlane = tmem_base + ((uint32_t)(quarter * 32) << 16);
-#pragma unroll 1
-            for (int c0 = 0; c0 < n16; c0 += 16) {
-                int v0[16], v1[16], v2[16];
-                gi_tmem_ld16(tlane + (uint32_t)c0, v0);
-                gi_tmem_ld16(tlane + (uint32_t)(n16 + c0), v1);
-                gi_tmem_ld16(tlane + (uint32_t)(2 * n16 + c0), v2);
-#pragma unroll
-                for (int k = 0; k < 16; ++k) {
-                    const double s = (double)v0[k] * 65536.0 + (double)v1[k] * 256.0 + (double)v2[k];      // exact: < 2^48
-                    dst[(long long)(c0 + k) * ldp] = s * (colmax[c0 + k] * (1.0 / 536870912.0));           // 2^16 2^-45
-                }
-            }
-            gu_tc_fence_before();
-            __syncwarp();
-            if (lane == 0) gu_mbar_arrive(acc_empty);
-            acc_phase ^= 1;
-        }
-    } else {
-        // ===== generators: two threads per row (16 points each); digits of round(2^23 G) into the three A planes =====
-        const int g = threadIdx.x - 6 * 32, r = g & 127, hf = g >> 7;
-        const uint32_t off = gi_row_half_offset(r, hf);
-        uint32_t stage = 0, phase = 0;
-        for (long long u = blockIdx.x; u < nunits; u += gridDim.x) {
-            const int q = (int)(u / ntiles), t = (int)(u % ntiles);
-            const long long j0 = (long long)q * chunk;
-            const int nst = (int)((min((long long)chunk, jpad - j0)) / GI_KS);
-            long long i = i_begin + (long long)t * GI_ROWS + r;
-            if (i >= i_end) i = i_end - 1;
+        for (int h = 0; h < 2; ++h) {
+            long long i = i_begin + (long long)t * GI_ROWS + r0 + 8 * h;
+            if (i >= i_end) i = i_end - 1;                              // rows past the end: computed, never read back
             const float4 a = pts[i];
-            const u64 ax2 = pack2(a.x, a.x), ay2 = pack2(a.y, a.y), az2 = pack2(a.z, a.z), magic2 = pack2(8388608.0f, 8388608.0f);
-            for (int kb = 0; kb < nst; ++kb) {
-                // the j-points arrive with the B image (global loads here stalled the 8 generator warps on L2 latency: long-scoreboard
-                // 4.2 of 7.6 warp-cycles per issue in the first version, profiles/r2_ncu_gi_gram_v2.txt)
-                gu_wait(&full_b[stage], phase, 19);
-                const ulonglong2* bj = reinterpret_cast<const ulonglong2*>(spts + stage * GI_PTS_BYTES) + hf * 16;     // 8 pair records
-                // g = round(2^23 G) sits in the mantissa of 2^23 + 2^23 G (one FMA; a float -> integer conversion would go through the
-                // quarter-rate XU pipe that MUFU.EX2 already loads): bytes 2, 1, 0 of the float ARE the digits a0 < 128, a1, a2.
-                // Two points per packed f32x2 instruction (the distance chain and the magic FMA), like the E-step kernels.
-                uint32_t gq[16];
-#pragma unroll
-                for (int pr = 0; pr < 8; ++pr) {
-                    const ulonglong2 bxy = bj[2 * pr];
-                    const u64 bz = bj[2 * pr + 1].x;
-                    const u64 dx = fsub2(ax2, bxy.x), dy = fsub2(ay2, bxy.y), dz = fsub2(az2, bz);
-                    const float2 u = unpack2(ffma2(dz, dz, ffma2(dy, dy, fmul2(dx, dx))));
-                    const u64 e = pack2(ex2(-u.x), ex2(-u.y));    // the same float32 G as the other kernels; G = 1 gives the digits (128, 0, 0)
-                    const float2 t = unpack2(ffma2(e, magic2, magic2));
-                    gq[2 * pr] = __float_as_uint(t.x);
-                    gq[2 * pr + 1] = __float_as_uint(t.y);
-                }
-                gu_wait(&empty[stage], phase ^ 1, 16);
-                unsigned char* sa = smem + stage * GI_STAGE_BYTES;
-#pragma unroll
-                for (int p = 0; p < 3; ++p) {
-                    const uint32_t sel = p == 0 ? 0x0062u : (p == 1 ? 0x0051u : 0x0040u);     // byte (2 - p) of both inputs
-                    uint4 w;
-                    w.x = __byte_perm(__byte_perm(gq[0], gq[1], sel), __byte_perm(gq[2], gq[3], sel), 0x5410u);
-                    w.y = __byte_perm(__byte_perm(gq[4], gq[5], sel), __byte_perm(gq[6], gq[7], sel), 0x5410u);
-                    w.z = __byte_perm(__byte_perm(gq[8], gq[9], sel), __byte_perm(gq[10], gq[11], sel), 0x5410u);
-                    w.w = __byte_perm(__byte_perm(gq[12], gq[13], sel), __byte_perm(gq[14], gq[15], sel), 0x5410u);
-                    *reinterpret_cast<uint4*>(sa + p * GI_PLANE + off) = w;
-                }
-                gu_fence_async_smem();
-                __syncwarp();
-                if (lane == 0) gu_mbar_arrive(&full_a[stage]);
-                if (++stage == GI_STAGES) { stage = 0; phase ^= 1; }
-            }
+            ax[h] = a.x; ay[h] = a.y; az[h] = a.z;
         }
-    }
-    gu_tc_fence_before();
-    __syncthreads();
-    if (warp == 1) gu_tmem_dealloc(tmem_base, 512);
-}
-
-constexpr int GI_TS_STAGES = 7;                        // the A ring in TMEM: 7 x 24 columns behind the 336 accumulator columns
-constexpr int GI_TS_GEN = 16;                          // generator warps (four threads per row of the tile)
-constexpr int GI_TS_THREADS = (6 + GI_TS_GEN) * 32;
-constexpr int GI_TS_STAGE_BYTES = 3 * GI_PLANE;         // shared memory per stage: the B image only
-constexpr int GI_TS_SMEM = GI_TS_STAGES * (GI_TS_STAGE_BYTES + GI_PTS_BYTES) + 1024 + 256;
-__device__ __forceinline__ void gi_mma_i8_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::i8 [%0], [%1], %2, %3, p;\n"
-        "}" ::"r"(d_tmem),
-        "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void gi_tmem_st2(uint32_t taddr, uint32_t w0, uint32_t w1) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x2.b32 [%0], {%1, %2};" ::"r"(taddr), "r"(w0), "r"(w1) : "memory");
-}
-// four consecutive 32-bit columns of this thread's TMEM lane
-__device__ __forceinline__ void gi_tmem_st4(uint32_t taddr, uint32_t w0, uint32_t w1, uint32_t w2, uint32_t w3) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1, %2, %3, %4};" ::"r"(taddr), "r"(w0), "r"(w1), "r"(w2), "r"(w3) : "memory");
-}
-
-// ---- the product, A operand in TENSOR MEMORY (tcgen05.mma ".ts" form) ---------------------------------------------------------------
-// Same algorithm, barriers and B pipeline as gi_gram_kernel; the generators write their digit rows with tcgen05.st into a ring of
-// TMEM columns (lane = row of the tile, 8 columns of 4 bytes per digit plane and stage) instead of shared memory, and the MMAs take A
-// from there.  Why: gi_gram_kernel is bound by the shared-memory port (generator STS + LDS 51 %, tensor operand reads 42 %,
-// profiles/r2_ncu_gi_gram_final.txt); this removes the 12 KB of STS and the 24 KB of A-operand reads per stage.
-// TMEM: accumulators in columns [0, 3 n16), the A ring behind 3 GI_NMAX: GI_TS_STAGES x 3 planes x 8 columns (336 + 168 = 504 <= 512).
-// A generator warp can only reach the 32 lanes of its quarter (warp id % 4): row = 32 (warp % 4) + lane, point group = (warp - 6) / 4.
-// one column pass: images = the stage images of gi_split_kernel (jpad / 32 of them); rows [i_begin, i_end) of G;
-// part[q][c][ii] (FP64) = colmax[c] 2^-45 sum_{j in chunk q} g_ij x_cj
-__global__ void __launch_bounds__(GI_TS_THREADS, 1)
-gi_gram_ts_kernel(const unsigned char* __restrict__ images, const float4* __restrict__ pts, const float4* __restrict__ pairs, long long jpad, int chunk,
-               long long i_begin,
-               long long i_end, int n16, const double* __restrict__ colmax, double* __restrict__ part, long long ldp) {
-    extern __shared__ __align__(1024) unsigned char gu_smem_raw[];
-    unsigned char* smem = gu_smem_raw;
-    unsigned char* spts = smem + GI_TS_STAGES * GI_TS_STAGE_BYTES;            // [GI_TS_STAGES][32] float4: the j-points of each stage
-    uint64_t* bars = reinterpret_cast<uint64_t*>(spts + GI_TS_STAGES * GI_PTS_BYTES);
-    uint64_t* full_a = bars;
-    uint64_t* full_b = bars + GI_TS_STAGES;
-    uint64_t* empty = bars + 2 * GI_TS_STAGES;
-    uint64_t* acc_full = bars + 3 * GI_TS_STAGES;
-    uint64_t* acc_empty = bars + 3 * GI_TS_STAGES + 1;
-    uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(bars + 3 * GI_TS_STAGES + 2);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const long long rows = i_end - i_begin;
-    const int ntiles = (int)((rows + GI_ROWS - 1) / GI_ROWS);
-    const int nq = (int)((jpad + chunk - 1) / chunk);
-    const long long nunits = (long long)ntiles * nq;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < GI_TS_STAGES; ++s) { mbar_init(&full_a[s], GI_TS_GEN); mbar_init(&full_b[s], 1); mbar_init(&empty[s], 1); }
-        mbar_init(acc_full, 1);
-        mbar_init(acc_empty, 4);
-        mbar_fence_init();
-    }
-    if (warp == 1) gu_tmem_alloc(tmem_base_slot, 512);
-    gu_tc_fence_before();
-    __syncthreads();
-    gu_tc_fence_after();
-    const uint32_t tmem_base = *tmem_base_slot;
-
-    if (warp == 0) {
-        // ===== TMA producer: the stage image (three digit planes of X for 32 points), one bulk copy =====
-        if (lane == 0) {
-            uint32_t stage = 0, phase = 0;
-            for (long long u = blockIdx.x; u < nunits; u += gridDim.x) {
-                const int q = (int)(u / ntiles);
-                const long long j0 = (long long)q * chunk;
-                const int nst = (int)((min((long long)chunk, jpad - j0)) / GI_KS);
-                const unsigned char* src = images + (j0 / GI_KS) * (3 * GI_PLANE);
-                for (int kb = 0; kb < nst; ++kb) {
-                    gu_wait(&empty[stage], phase ^ 1, 11);
-                    mbar_expect_tx(&full_b[stage], (uint32_t)(3 * GI_PLANE + GI_PTS_BYTES));
-                    tma_load_1d(smem + stage * GI_TS_STAGE_BYTES, src + (long long)kb * (3 * GI_PLANE), (uint32_t)(3 * GI_PLANE),
-                                &full_b[stage]);
-                    tma_load_1d(spts + stage * GI_PTS_BYTES, pairs + j0 + (long long)kb * GI_KS, (uint32_t)GI_PTS_BYTES, &full_b[stage]);
-                    if (++stage == GI_TS_STAGES) { stage = 0; phase ^= 1; }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ===== MMA issuer: level l = s + t accumulates a_s x b_t; the whole warp walks the pipeline, one elected lane issues =====
-        {
-            const uint32_t idesc = gi_instr_desc(n16);
-            uint32_t stage = 0, phase = 0, acc_phase = 0;
-            for (long long u = blockIdx.x; u < nunits; u += gridDim.x) {
-                const int q = (int)(u / ntiles);
-                const long long j0 = (long long)q * chunk;
-                const int nst = (int)((min((long long)chunk, jpad - j0)) / GI_KS);
-                gu_wait(acc_empty, acc_phase ^ 1, 12);
-                gu_tc_fence_after();
-                for (int kb = 0; kb < nst; ++kb) {
-                    gu_wait(&full_a[stage], phase, 13);
-                    gu_wait(&full_b[stage], phase, 14);
-                    gu_tc_fence_after();
-                    const uint32_t sb = smem_u32(smem) + stage * GI_TS_STAGE_BYTES;
-                    const uint32_t ta = tmem_base + (uint32_t)(3 * GI_NMAX + stage * 24);       // this stage's three A planes (8 columns each)
-                    const uint32_t first = kb != 0 ? 1u : 0u;
-                    if (gu_elect_one()) {
-                        uint64_t b[3];
+        int acc0[32] = {}, acc1[32] = {}, acc2[32] = {};
+        for (int kb = 0; kb < nst; ++kb) {
+            mbar_wait(&full[stage], phase);
+            const float4* bj = spts + stage * GI_KS;
+            // g = round(2^23 G) sits in the mantissa of 2^23 + 2^23 G (one FMA; a float -> integer conversion would go through the
+            // quarter-rate pipe that MUFU.EX2 already loads): bytes 2, 1, 0 of the float ARE the digits a0 < 128, a1, a2.
+            // gq[h][s]: row r0 + 8 h, point kq + s (s < 4) or 16 + kq + s - 4
+            uint32_t gq[2][8];
 #pragma unroll
-                        for (int p = 0; p < 3; ++p) b[p] = gi_smem_desc(sb + p * GI_PLANE);
-                        gi_mma_i8_ts(tmem_base, ta, b[0], idesc, first);
-                        gi_mma_i8_ts(tmem_base + (uint32_t)n16, ta, b[1], idesc, first);
-                        gi_mma_i8_ts(tmem_base + (uint32_t)n16, ta + 8, b[0], idesc, 1u);
-                        gi_mma_i8_ts(tmem_base + (uint32_t)(2 * n16), ta, b[2], idesc, first);
-                        gi_mma_i8_ts(tmem_base + (uint32_t)(2 * n16), ta + 8, b[1], idesc, 1u);
-                        gi_mma_i8_ts(tmem_base + (uint32_t)(2 * n16), ta + 16, b[0], idesc, 1u);
-                        gu_commit(&empty[stage]);
-                        if (kb == nst - 1) gu_commit(acc_full);
-                    }
-                    __syncwarp();
-                    if (++stage == GI_TS_STAGES) { stage = 0; phase ^= 1; }
-                }
-                acc_phase ^= 1;
-            }
-        }
-    } else if (warp < 6) {
-        // ===== epilogue: join the three levels in FP64 (exact), scale, store the chunk partial =====
-        const int quarter = warp & 3;
-        uint32_t acc_phase = 0;
-        for (long long u = blockIdx.x; u < nunits; u += gridDim.x) {
-            const int q = (int)(u / ntiles), t = (int)(u % ntiles);
-            gu_wait_relaxed(acc_full, acc_phase, 15);
-            gu_tc_fence_after();
-            const long long ii = (long long)t * GI_ROWS + quarter * 32 + lane;
-            double* dst = part + (long long)q * n16 * ldp + ii;
-            const uint32_t tlane = tmem_base + ((uint32_t)(quarter * 32) << 16);
-#pragma unroll 1
-            for (int c0 = 0; c0 < n16; c0 += 16) {
-                int v0[16], v1[16], v2[16];
-                gi_tmem_ld16(tlane + (uint32_t)c0, v0);
-                gi_tmem_ld16(tlane + (uint32_t)(n16 + c0), v1);
-                gi_tmem_ld16(tlane + (uint32_t)(2 * n16 + c0), v2);
+            for (int s = 0; s < 8; ++s) {
+                const float4 b = bj[(s < 4 ? 0 : 16) + kq + (s & 3)];
 #pragma unroll
-                for (int k = 0; k < 16; ++k) {
-                    const double s = (double)v0[k] * 65536.0 + (double)v1[k] * 256.0 + (double)v2[k];      // exact: < 2^48
-                    dst[(long long)(c0 + k) * ldp] = s * (colmax[c0 + k] * (1.0 / 536870912.0));           // 2^16 2^-45
+                for (int h = 0; h < 2; ++h) {
+                    const float dx = __fsub_rn(ax[h], b.x), dy = __fsub_rn(ay[h], b.y), dz = __fsub_rn(az[h], b.z);
+                    const float uu = __fmaf_rn(dz, dz, __fmaf_rn(dy, dy, __fmul_rn(dx, dx)));
+                    const float e = ex2(-uu);                   // the same float32 G as the other kernels; G = 1 gives the digits (128, 0, 0)
+                    gq[h][s] = __float_as_uint(__fmaf_rn(e, 8388608.0f, 8388608.0f));
                 }
             }
-            gu_tc_fence_before();
+            uint32_t a[3][4];
+#pragma unroll
+            for (int p = 0; p < 3; ++p) {
+                const uint32_t sel = p == 0 ? 0x0062u : (p == 1 ? 0x0051u : 0x0040u);     // byte (2 - p) of both inputs
+#pragma unroll
+                for (int reg = 0; reg < 4; ++reg) {
+                    const uint32_t* g = &gq[reg & 1][(reg >> 1) * 4];
+                    a[p][reg] = __byte_perm(__byte_perm(g[0], g[1], sel), __byte_perm(g[2], g[3], sel), 0x5410u);
+                }
+            }
+            const uint32_t sb = smem_u32(planes + stage * 3 * GI_PLANE);
+            const uint64_t b0 = gi_smem_desc(sb), b1 = gi_smem_desc(sb + GI_PLANE), b2 = gi_smem_desc(sb + 2 * GI_PLANE);
+            const int more = kb != 0;
+            gi_wgmma_fence();
+            gi_mma(acc0, a[0], b0, more);
+            gi_mma(acc1, a[0], b1, more);
+            gi_mma(acc1, a[1], b0, 1);
+            gi_mma(acc2, a[0], b2, more);
+            gi_mma(acc2, a[1], b1, 1);
+            gi_mma(acc2, a[2], b0, 1);
+            gi_wgmma_commit();
+            gi_wgmma_wait_all();
             __syncwarp();
-            if (lane == 0) gu_mbar_arrive(acc_empty);
-            acc_phase ^= 1;
+            if (lane == 0) gi_mbar_arrive(&empty[stage]);
+            if (++stage == GI_STAGES) { stage = 0; phase ^= 1; }
         }
-    } else {
-        // ===== generators: FOUR threads per row (8 points each), 16 warps: four per scheduler instead of two -- the 8-warp version
-        // issued at half the peak rate with every pipe below 45 % (latency, not throughput).  Digits of round(2^23 G) -> TMEM =====
-        const int quarter = warp & 3, r = quarter * 32 + lane, part = (warp - 6) >> 2;          // part: which 8 of the stage's 32 points
-        uint32_t stage = 0, phase = 0;
-        for (long long u = blockIdx.x; u < nunits; u += gridDim.x) {
-            const int q = (int)(u / ntiles), t = (int)(u % ntiles);
-            const long long j0 = (long long)q * chunk;
-            const int nst = (int)((min((long long)chunk, jpad - j0)) / GI_KS);
-            long long i = i_begin + (long long)t * GI_ROWS + r;
-            if (i >= i_end) i = i_end - 1;
-            const float4 a = pts[i];
-            const u64 ax2 = pack2(a.x, a.x), ay2 = pack2(a.y, a.y), az2 = pack2(a.z, a.z), magic2 = pack2(8388608.0f, 8388608.0f);
-            for (int kb = 0; kb < nst; ++kb) {
-                gu_wait(&full_b[stage], phase, 19);                // the j-points arrive with the B image
-                const ulonglong2* bj = reinterpret_cast<const ulonglong2*>(spts + stage * GI_PTS_BYTES) + part * 8;     // 4 pair records
-                // g = round(2^23 G) sits in the mantissa of 2^23 + 2^23 G (one FMA; a float -> integer conversion would go through the
-                // quarter-rate XU pipe that MUFU.EX2 already loads): bytes 2, 1, 0 of the float ARE the digits a0 < 128, a1, a2.
-                uint32_t gq[8];
+        // ===== epilogue: join the three levels in FP64 (exact), scale, store the chunk partial =====
+        const long long ii = (long long)t * GI_ROWS + r0;
+        double* dst = part + (long long)q * GI_N * ldp + ii;
 #pragma unroll
-                for (int pr = 0; pr < 4; ++pr) {
-                    const ulonglong2 bxy = bj[2 * pr];
-                    const u64 bz = bj[2 * pr + 1].x;
-                    const u64 dx = fsub2(ax2, bxy.x), dy = fsub2(ay2, bxy.y), dz = fsub2(az2, bz);
-                    const float2 uu = unpack2(ffma2(dz, dz, ffma2(dy, dy, fmul2(dx, dx))));
-                    const u64 e = pack2(ex2(-uu.x), ex2(-uu.y));  // the same float32 G as the other kernels; G = 1 gives the digits (128, 0, 0)
-                    const float2 tt = unpack2(ffma2(e, magic2, magic2));
-                    gq[2 * pr] = __float_as_uint(tt.x);
-                    gq[2 * pr + 1] = __float_as_uint(tt.y);
-                }
-                gu_wait(&empty[stage], phase ^ 1, 16);
-                gu_tc_fence_after();                               // the MMAs that read this slot last have completed (tcgen05.commit)
-                const uint32_t ta = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(3 * GI_NMAX + stage * 24 + part * 2);
+        for (int i = 0; i < 8; ++i)
 #pragma unroll
-                for (int p = 0; p < 3; ++p) {
-                    const uint32_t sel = p == 0 ? 0x0062u : (p == 1 ? 0x0051u : 0x0040u);     // byte (2 - p) of both inputs
-                    const uint32_t w0 = __byte_perm(__byte_perm(gq[0], gq[1], sel), __byte_perm(gq[2], gq[3], sel), 0x5410u);
-                    const uint32_t w1 = __byte_perm(__byte_perm(gq[4], gq[5], sel), __byte_perm(gq[6], gq[7], sel), 0x5410u);
-                    gi_tmem_st2(ta + (uint32_t)(p * 8), w0, w1);       // this row's 8 bytes of plane p: 2 columns
+            for (int h = 0; h < 2; ++h) {
+                const int c = 8 * i + 2 * (lane & 3) + h;
+                const double sc = colmax[c] * (1.0 / 536870912.0);                                 // 2^16 2^-45
+#pragma unroll
+                for (int rr = 0; rr < 2; ++rr) {
+                    const int k = 4 * i + 2 * rr + h;
+                    const double s = (double)acc0[k] * 65536.0 + (double)acc1[k] * 256.0 + (double)acc2[k];     // exact: < 2^48
+                    dst[(long long)c * ldp + 8 * rr] = s * sc;
                 }
-                asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-                gu_tc_fence_before();
-                __syncwarp();
-                if (lane == 0) gu_mbar_arrive(&full_a[stage]);
-                if (++stage == GI_TS_STAGES) { stage = 0; phase ^= 1; }
             }
-        }
     }
-    gu_tc_fence_before();
-    __syncthreads();
-    if (warp == 1) gu_tmem_dealloc(tmem_base, 512);
-}
-
-// ---- layout probe: D[128][n16] (int32) = A[128][32] (u8) x B[n16][32]^T (s8), through the conventions above -------------------------
-__global__ void __launch_bounds__(128, 1)
-gi_layout_probe_kernel(const __grid_constant__ CUtensorMap bmap, const unsigned char* __restrict__ A, int n16, int* __restrict__ D) {
-    extern __shared__ __align__(1024) unsigned char gu_smem_raw[];
-    unsigned char* smem = gu_smem_raw;
-    unsigned char* sa = smem;
-    unsigned char* sb = smem + 4096;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 4096 + 8192);
-    uint32_t* slot = reinterpret_cast<uint32_t*>(bars + 2);
-    const int warp = threadIdx.x >> 5, r = threadIdx.x;
-    if (threadIdx.x == 0) { mbar_init(&bars[0], 1); mbar_init(&bars[1], 1); mbar_fence_init(); }
-    if (warp == 0) gu_tmem_alloc(slot, 256);
-    gu_tc_fence_before();
-    __syncthreads();
-    gu_tc_fence_after();
-    const uint32_t tmem_base = *slot;
-    if (threadIdx.x == 0) {
-        mbar_expect_tx(&bars[0], (uint32_t)(n16 * 32));
-        gu_tma_load_2d(sb, &bmap, 0, 0, &bars[0]);
-    }
-#pragma unroll
-    for (int h = 0; h < 2; ++h) *reinterpret_cast<uint4*>(sa + gi_row_half_offset(r, h)) = *reinterpret_cast<const uint4*>(A + r * 32 + 16 * h);
-    gu_fence_async_smem();
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        gu_wait(&bars[0], 0, 17);
-        gu_tc_fence_after();
-        gi_mma_i8(tmem_base, gi_smem_desc(smem_u32(sa)), gi_smem_desc(smem_u32(sb)), gi_instr_desc(n16), 0u);
-        gu_commit(&bars[1]);
-    }
-    gu_wait(&bars[1], 0, 18);
-    gu_tc_fence_after();
-    for (int c0 = 0; c0 < n16; c0 += 16) {
-        int v[16];
-        gi_tmem_ld16(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0, v);
-        for (int k = 0; k < 16; ++k) D[r * n16 + c0 + k] = v[k];
-    }
-    gu_tc_fence_before();
-    __syncthreads();
-    if (warp == 0) gu_tmem_dealloc(tmem_base, 256);
-}
-
-// the same probe with A in tensor memory (tcgen05.st by the owning thread, ".ts" MMA)
-__global__ void __launch_bounds__(128, 1)
-gi_layout_probe_ts_kernel(const __grid_constant__ CUtensorMap bmap, const unsigned char* __restrict__ A, int n16, int* __restrict__ D) {
-    extern __shared__ __align__(1024) unsigned char gu_smem_raw[];
-    unsigned char* smem = gu_smem_raw;
-    unsigned char* sb = smem;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 8192);
-    uint32_t* slot = reinterpret_cast<uint32_t*>(bars + 2);
-    const int warp = threadIdx.x >> 5, r = threadIdx.x;
-    if (threadIdx.x == 0) { mbar_init(&bars[0], 1); mbar_init(&bars[1], 1); mbar_fence_init(); }
-    if (warp == 0) gu_tmem_alloc(slot, 512);
-    gu_tc_fence_before();
-    __syncthreads();
-    gu_tc_fence_after();
-    const uint32_t tmem_base = *slot;
-    if (threadIdx.x == 0) {
-        mbar_expect_tx(&bars[0], (uint32_t)(n16 * 32));
-        gu_tma_load_2d(sb, &bmap, 0, 0, &bars[0]);
-    }
-    const uint4 lo = *reinterpret_cast<const uint4*>(A + r * 32), hi = *reinterpret_cast<const uint4*>(A + r * 32 + 16);
-    const uint32_t ta = tmem_base + ((uint32_t)(warp * 32) << 16) + 256u;          // A in columns 256..263
-    gi_tmem_st4(ta, lo.x, lo.y, lo.z, lo.w);
-    gi_tmem_st4(ta + 4, hi.x, hi.y, hi.z, hi.w);
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-    gu_tc_fence_before();
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        gu_wait(&bars[0], 0, 27);
-        gu_tc_fence_after();
-        gi_mma_i8_ts(tmem_base, tmem_base + 256u, gi_smem_desc(smem_u32(sb)), gi_instr_desc(n16), 0u);
-        gu_commit(&bars[1]);
-    }
-    gu_wait(&bars[1], 0, 28);
-    gu_tc_fence_after();
-    for (int c0 = 0; c0 < n16; c0 += 16) {
-        int v[16];
-        gi_tmem_ld16(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0, v);
-        for (int k = 0; k < 16; ++k) D[r * n16 + c0 + k] = v[k];
-    }
-    gu_tc_fence_before();
-    __syncthreads();
-    if (warp == 0) gu_tmem_dealloc(tmem_base, 512);
-}
-
-// tensor map over byte planes: [rows][ld] bytes, box {32, box_rows}, 32-byte swizzle
-inline int gi_make_map(CUtensorMap* map, const void* base, long long ld, long long rows, int box_rows) {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess || !fn) return -1;
-    const cuuint64_t dims[2] = {(cuuint64_t)ld, (cuuint64_t)rows};
-    const cuuint64_t strides[1] = {(cuuint64_t)ld};
-    const cuuint32_t box[2] = {(cuuint32_t)GI_KS, (cuuint32_t)box_rows};
-    const cuuint32_t estr[2] = {1, 1};
-    const CUresult r = reinterpret_cast<gu_encode_fn>(fn)(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(base), dims, strides, box, estr,
-                                                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_32B,
-                                                          CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    return r == CUDA_SUCCESS ? 0 : (int)r;
 }
 
 }  // namespace cpd

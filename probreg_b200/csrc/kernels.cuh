@@ -1,4 +1,4 @@
-// kernels.cuh -- sm_100a device code of the CPD EM hot path.
+// kernels.cuh -- sm_90a (H100) device code of the CPD EM hot path.
 //
 // What is computed (reference: probreg/cpd.py:71-88, restated in oracle/cpd_oracle.py):
 //   K_mn = exp(-|yhat_m - x_n|^2 / (2 sigma^2)),  den_n = sum_m K_mn (+ eps32 if 0) + c,
@@ -30,7 +30,7 @@
 
 namespace cpd {
 
-// tunables (tools/tune.sh builds variants with -D...; the defaults are the measured best)
+// tunables (tools/tune.sh builds variants with -D...; the defaults are not tuned for the H100)
 #ifndef CPD_RI1
 #define CPD_RI1 4
 #endif
@@ -59,7 +59,7 @@ constexpr int UNROLL1 = CPD_UNROLL1, UNROLL2 = CPD_UNROLL2;
 constexpr int THREADS = 256;           // threads per CTA in both passes
 constexpr int RI1 = CPD_RI1, RI2 = CPD_RI2;            // i-points held in registers per thread (pass 1 / pass 2)
 constexpr int ITILE1 = THREADS * RI1, ITILE2 = THREADS * RI2;   // i-points per CTA
-constexpr int NPAIR1 = RI1 / 2, NPAIR2 = RI2 / 2;      // i-points are processed as packed f32x2 pairs (FADD2 / FFMA2)
+constexpr int NPAIR1 = RI1 / 2, NPAIR2 = RI2 / 2;      // i-points are processed in pairs (fsub2 / ffma2 below)
 #ifndef CPD_P1_STAGE
 #define CPD_P1_STAGE 512
 #endif
@@ -69,7 +69,7 @@ constexpr int NPAIR1 = RI1 / 2, NPAIR2 = RI2 / 2;      // i-points are processed
 constexpr int P1_STAGE = CPD_P1_STAGE;   // sources per TMA stage in pass 1 (32 B records -> 16 KB); a multiple of 256
 constexpr int P2_STAGE = CPD_P2_STAGE;   // targets per TMA stage in pass 2 (48 B records -> 24 KB); a multiple of 256
 static_assert(P1_STAGE % 256 == 0 && P2_STAGE % 256 == 0 && P1_STAGE >= 256 && P2_STAGE >= 256, "stage sizes are multiples of 256");
-constexpr int P1_REC = 32, P2_REC = 48;    // bytes per streamed j-record (coordinates duplicated for f32x2)
+constexpr int P1_REC = 32, P2_REC = 48;    // bytes per streamed j-record (coordinates duplicated for the pair loops)
 #ifndef CPD_NSTAGE
 #define CPD_NSTAGE 3
 #endif
@@ -100,8 +100,8 @@ constexpr double EPS32 = 1.1920928955078125e-07;
 // with v_m = sum_n P_mn (x_n - T(y_m)) the weighted residual of source m and y~ = y - cy.
 enum { RM_NP = 0, RM_SY = 1, RM_C = 4, RM_V1 = 10, RM_VY = 13, RM_SRC = 22, RM_SRR = 22, RM_NPT = 23, RM_TGT = 2,
        RM_COUNT = 24, MOM_PAD = 32 };
-// Moments of the API-faithful M-step (cpd_mstep: a caller-supplied EstepResult; SURVEY appendix A.3
-// extended with the pt1-side sums the reference uses)
+// Moments of the API-faithful M-step (cpd_mstep: a caller-supplied EstepResult;
+// the reference's sums extended with the pt1-side sums the reference uses)
 enum { MOM_NP = 0, MOM_SX = 1, MOM_SY = 4, MOM_B = 7, MOM_C = 16, MOM_NPT = 22, MOM_SXT = 23, MOM_TXX = 26,
        MOM_COUNT = 27, MOM_SRC = 22, MOM_TGT = 5 };
 
@@ -134,7 +134,7 @@ struct DevState {
     int err;             // set by a kernel that gave up waiting for a peer (P2P exchange); checked by the host
 };
 
-// One-shot all-reduce of the 32 moment doubles over NVLink peer memory (SURVEY section 8e): every rank owns
+// One-shot all-reduce of the 32 moment doubles over NVLink peer memory: every rank owns
 // a mailbox that its peers write into; slots are double-buffered by exchange parity, flags carry the
 // exchange sequence number (monotonic, never reset), sums are formed in rank order => bit-identical on all ranks.
 constexpr int P2P_MAX = 16;
@@ -162,16 +162,28 @@ __device__ __forceinline__ float ex2(float x) {
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
 }
-// packed FP32 pairs (sm_100 FADD2 / FMUL2 / FFMA2): one issue slot for two lanes' worth of FP32 work.
-// The E-step is issue-bound in scalar form (19 FP32-pipe + 2 MUFU slots per pair and iteration);
-// packed, the same work takes 10.5 slots and the MUFU / FMA pipes become the limit (profiles/).
+// FP32 pairs: two i-points travel together through the pair loops (one 64-bit register pair, one 8-byte shared-memory load
+// per j-coordinate for both).  Hopper has no packed FP32 instructions, so each helper is two scalar IEEE operations with the
+// rounding of the corresponding f32x2 instruction (the _rn intrinsics also keep the compiler from contracting them).
 typedef unsigned long long u64;
-__device__ __forceinline__ u64 fsub2(u64 a, u64 b) { u64 d; asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
-__device__ __forceinline__ u64 fadd2(u64 a, u64 b) { u64 d; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
-__device__ __forceinline__ u64 fmul2(u64 a, u64 b) { u64 d; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
-__device__ __forceinline__ u64 ffma2(u64 a, u64 b, u64 c) { u64 d; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c)); return d; }
 __device__ __forceinline__ u64 pack2(float lo, float hi) { u64 r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi)); return r; }
 __device__ __forceinline__ float2 unpack2(u64 v) { float2 r; asm("mov.b64 {%0, %1}, %2;" : "=f"(r.x), "=f"(r.y) : "l"(v)); return r; }
+__device__ __forceinline__ u64 fsub2(u64 a, u64 b) {
+    const float2 x = unpack2(a), y = unpack2(b);
+    return pack2(__fsub_rn(x.x, y.x), __fsub_rn(x.y, y.y));
+}
+__device__ __forceinline__ u64 fadd2(u64 a, u64 b) {
+    const float2 x = unpack2(a), y = unpack2(b);
+    return pack2(__fadd_rn(x.x, y.x), __fadd_rn(x.y, y.y));
+}
+__device__ __forceinline__ u64 fmul2(u64 a, u64 b) {
+    const float2 x = unpack2(a), y = unpack2(b);
+    return pack2(__fmul_rn(x.x, y.x), __fmul_rn(x.y, y.y));
+}
+__device__ __forceinline__ u64 ffma2(u64 a, u64 b, u64 c) {
+    const float2 x = unpack2(a), y = unpack2(b), z = unpack2(c);
+    return pack2(__fmaf_rn(x.x, y.x, z.x), __fmaf_rn(x.y, y.y, z.y));
+}
 __device__ __forceinline__ unsigned long long globaltimer_ns() {
     unsigned long long t;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
@@ -436,7 +448,7 @@ __device__ __forceinline__ float box_gap2(const float* __restrict__ wbox, const 
 // terms are first summed in groups of GRP from zero and the group sums joined: a two-level FP32 summation.
 // Why: adding thousands of tiny terms one by one to a partial sum that already holds a dominant term drops
 // them (absorption), a SYSTEMATIC loss that does not average out -- measured -1.2e-6 on sigma2 with a flat
-// 64-term sum, -2e-6 with 128 (profiles/r1_precision_subchunk.txt).
+// 64-term sum, -2e-6 with 128.
 // WGT: every source carries a weight 2^-la (la >= 0) in the spare half of its z-record; t' = u - o + la, added LAST so that
 // pass 2 (which adds the same la after the same FMA chain) sees bit-identical exponents (the BCPD E-step, bcpd.py:53-66).
 template <bool WGT>
@@ -696,7 +708,7 @@ pass1_kernel(const float4* __restrict__ ipts, int ni, const float4* __restrict__
 //   L      = log2(den) = log2(2^log2S + c)          c = (2 pi s2)^(D/2) w/(1-w) M/N  (cpd.py:78-79)
 //   pt1    = 2^(log2S - L)                          (cpd.py:85; == 1 when w == 0)
 //   rn     = 2^(-omin) / den = 2^-(L + omin)        P_mn = 2^(omin - u_mn) * rn in pass 2
-//   record = {bx,bx,by,by},{bz,bz,-omin,-omin},{rn,rn,0,0}   (48 B, duplicated for the f32x2 inner loop)
+//   record = {bx,bx,by,by},{bz,bz,-omin,-omin},{rn,rn,0,0}   (48 B, duplicated for the pair inner loop)
 //            dead / padding: -omin = +inf (so 2^-(u - omin) == 0), rn = 0
 // and the target-side moments: Srr = sum_n SU_n rn_n (= sum_mn P_mn u_mn), Npt = sum pt1.
 // ---------------------------------------------------------------------------------------------
@@ -1232,7 +1244,7 @@ __device__ inline void mstep_solve_residual(DevState* st, const double* __restri
 }
 
 // The M-step of the fused loop on a shared-memory copy of the state: thread 0 alone walking DevState and the moments in global
-// memory paid one L2 round trip per field (~50 dependent loads: 20 of the kernel's 33 us, profiles/r2_ncu_shard_1of8.txt).
+// memory paid one L2 round trip per field (~50 dependent loads).
 // All threads of the calling block must enter; `mom` may be global or shared.
 __device__ __forceinline__ void mstep_staged(DevState* st, const double* mom) {
     __shared__ DevState sst;
@@ -1590,7 +1602,7 @@ imq_kernel_kernel(const float* __restrict__ x, long long nx, const float* __rest
 }
 
 // ---------------------------------------------------------------------------------------------
-// Non-rigid CPD, dense G (probreg/cpd.py:247-303, transformation.py:81-102) -- SURVEY section 8(f) row 1.
+// Non-rigid CPD, dense G (probreg/cpd.py:247-303, transformation.py:81-102).
 // G stays on the device as float32 (the reference's _math.rbf_kernel is float32, cc/types.h:19); the
 // M x M system of cpd.py:296 is assembled in FP64 and handed to cuSOLVER's LU (a plain library solve).
 // ---------------------------------------------------------------------------------------------
@@ -1744,7 +1756,7 @@ nr_sigma_kernel(DevState* st, const double* __restrict__ part, int nb, const dou
 }
 
 // ---------------------------------------------------------------------------------------------
-// Direct Gauss transform (probreg/gauss_transform.py:10-16; SURVEY section 8(f) row 2): the same pair kernel as
+// Direct Gauss transform (probreg/gauss_transform.py:10-16): the same pair kernel as
 // pass 1 without the normalisation:  out[c][i] = sum_j w[c][j] exp(-|t_i - s_j|^2 / h^2),  up to GT_K weight
 // vectors per sweep.  Coordinates arrive centred and scaled by sqrt(log2 e)/h, so the exponential is 2^(-u).
 // FP32 pair maths, 32-term FP32 groups, FP64 beyond.  Exact (the reference's default for h >= 0.01 is the
@@ -1818,7 +1830,7 @@ probe_mufu_kernel(float* out, int iters, float seed) {
     for (int k = 0; k < 8; ++k) s += a[k];
     if (s == 123.456f) out[0] = s;
 }
-// packed FP32 (FFMA2): 2 FMAs per lane per instruction -- does it raise the FLOP rate or only save issue slots?
+// the pair helpers (ffma2: two scalar FMAs on sm_90): the FMA rate the pair loops can reach
 __global__ void __launch_bounds__(256)
 probe_ffma2_kernel(float* out, int iters, float seed) {
     u64 a[8];
@@ -1834,7 +1846,7 @@ probe_ffma2_kernel(float* out, int iters, float seed) {
     for (int k = 0; k < 8; ++k) { const float2 v = unpack2(a[k]); s += v.x + v.y; }
     if (s == 123.456f) out[0] = s;
 }
-// FFMA2 and scalar FFMA interleaved: is there capacity (an idle "lite" FMA pipe) that packed code leaves unused?
+// pair FMAs and single FMAs interleaved
 __global__ void __launch_bounds__(256)
 probe_ffma_mixed_kernel(float* out, int iters, float seed) {
     u64 a[6];

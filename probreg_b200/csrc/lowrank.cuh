@@ -1,5 +1,5 @@
-// lowrank.cuh -- non-rigid CPD with a rank-K factorisation of the RBF Gram matrix (SURVEY section 8(f) row 1,
-// BASELINE configuration 5: N = M = 50k, K = 200).
+// lowrank.cuh -- non-rigid CPD with a rank-K factorisation of the RBF Gram matrix
+// (BASELINE configuration 5: N = M = 50k, K = 200).
 //
 // Reference: NonRigidCPD._maximization_step (probreg/cpd.py:284-303) solves the dense M x M system
 //     (diag(p1) G + lmd sigma2 I) W = px - diag(p1) Y,        G_ij = exp(-|y_i - y_j|^2 / (2 beta))   (cc/math_utils.cc:17-19)
@@ -12,7 +12,7 @@
 //     Z  = Bc Q^T W  solves the K x K system  (c I + Bc S) Z = Bc R,   S = Q^T diag(p1) Q,  R = Q^T F
 //     T  = Y + G W ~= Y + Q Z
 // (Woodbury written without Bc^-1, so numerically rank-deficient Q -- zero columns -- is harmless.)
-// Since round 2 the iteration runs on the factor Qt = Q L, Bc ~= L L^T, whose K x K system is symmetric positive definite and is
+// The iteration runs on the factor Qt = Q L, Bc ~= L L^T, whose K x K system is symmetric positive definite and is
 // solved by one CTA (lr_spd_form in host_nonrigid.inl, lr_pchol_kernel / lr_spd_solve_kernel below); the unsymmetric system above
 // with cuSOLVER's LU remains for K > LR_SPD_MAX_RANK and as the cross-check (CPD_B200_LR_CORE=lu).
 // Parity: against the dense device path / the numpy oracle at small M (tests); at K = M the two coincide up to rounding.
@@ -110,7 +110,7 @@ lr_gram_apply_kernel(const float4* __restrict__ pts, long long m, long long mpad
 
 // ---- orthonormalisation of the columns of X (classical Gram-Schmidt, every column projected twice) ---------------------
 // part[s][k] = <X_k, X_j> over the s-th of LR_SLICES point slices, for k = k_first .. j (the last one is |X_j|^2).
-// One CTA per {k, slice}: a single CTA per k would stream 2 M doubles through one SM (~20 us at M = 50k, whatever j is);
+// One CTA per {k, slice}: a single CTA per k would stream 2 M doubles through one SM, whatever j is;
 // consumers add the slices in a fixed order, so the result is reproducible.
 __global__ void __launch_bounds__(THREADS)
 lr_dots_kernel(const double* __restrict__ X, long long m, long long ld, int j, int k_first, int stride /* rank + 1 */,
@@ -232,7 +232,7 @@ lr_panel_gram_kernel(const double* __restrict__ X, long long m, long long ld, in
 //   mode 0 (step d):  scale2 from (b) turns the diagonal of W back into the column's remaining norm^2 in arrival units; the
 //       column-wise rule (kept iff that is > 1e-28 n0) decides.  Dropped columns get a zero column in T and stay exactly zero.
 // The factorisation is right-looking on one warp (lane = column): 16 steps of a few operations instead of one thread walking
-// ~3000 dependent FP64 operations (75 us in the first version).
+// ~3000 dependent FP64 operations.
 constexpr int LR_CHOL_THREADS = 1024;   // 4 threads per Gram entry for the merge of the block partials
 __global__ void __launch_bounds__(LR_CHOL_THREADS)
 lr_panel_chol_kernel(const double* __restrict__ part, int nblk, int np, double* __restrict__ n0, int mode, double* __restrict__ scale2,
@@ -242,7 +242,7 @@ lr_panel_chol_kernel(const double* __restrict__ part, int nblk, int np, double* 
     __shared__ int live[LR_PANEL];          // 1: part of the factorisation, 2: projected and rescaled only, 0: dropped
     const int tid = threadIdx.x, t = tid & 255, a = t / LR_PANEL, b = t % LR_PANEL, lane4 = tid >> 8;
     {   // merge: thread group lane4 takes the blocks lane4, lane4 + 4, ...; the four sums are joined in a fixed order (the merge
-        // used to be 196 dependent L2 round trips on 256 threads: 25 of the kernel's 30 us)
+        // of one thread per entry would be 196 dependent L2 round trips)
         double s = 0.0;
 #pragma unroll 8
         for (int k = lane4; k < nblk; k += 4) s += part[(size_t)k * (LR_PANEL * LR_PANEL) + t];
@@ -519,10 +519,10 @@ lr_system_kernel(const double* __restrict__ Bc, const double* __restrict__ S, co
 // against the unsymmetric (c I + Bc S) Z = Bc R of the orthonormal factor.  lr_spd_solve_kernel solves it in ONE CTA: the lower
 // triangle of  c I + St  with the three right-hand sides appended as rows K .. K+2 lives in shared memory (packed by rows,
 // (K+3)(K+4)/2 doubles: 166 KB at K = 200, plus the panel buffer), a blocked LDL^T factorisation runs over it (see the kernel) -- the
-// appended rows come out as the forward substitution -- then the back substitution in registers.  0.17 ms per M-step at K = 200;
-// cuSOLVER's LU of the unsymmetric form took 0.48 ms (getrf is a single 256-thread CTA there, plus laswp and two trsm).
-// (An eigen-decomposition of Bc would serve as well as the Cholesky factor; cusolverDnXsyevd takes 1.8 ms at K = 200 but 38 s on
-//  its first call in a process on the B200 box -- profiles/r2_syevd_probe.txt -- so the factor is computed here.)
+// appended rows come out as the forward substitution -- then the back substitution in registers.  It replaces cuSOLVER's LU of
+// the unsymmetric form (getrf is a single 256-thread CTA there, plus laswp and two trsm), which stays selectable with
+// CPD_B200_LR_CORE=lu.  (An eigen-decomposition of Bc would serve as well as the Cholesky factor; cusolverDnXsyevd's first call
+// in a process is costly, so the factor is computed here.)
 constexpr int LR_SPD_THREADS = 512;           // 128 registers per thread: phase 1 keeps an 8 x 8 block in registers
 constexpr int LR_SPD_B = 8;                  // columns per panel: two barriers per LR_SPD_B columns
 constexpr int LR_SPD_RG = 4;                 // rows per warp pass in the trailing update

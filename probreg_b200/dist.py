@@ -1,7 +1,7 @@
 """Multi-GPU plumbing: one process per GPU, targets sharded, sources replicated.
 
-The reference has no distributed path at all; this is the B200-side design of SURVEY section
-8(e).  ``den_n`` is a sum over sources for a fixed target, so with the sources replicated the
+The reference has no distributed path at all; this is the multi-GPU design.
+``den_n`` is a sum over sources for a fixed target, so with the sources replicated the
 first E-step pass needs no communication; the second pass yields per-rank partial sums of the
 M-step moments, which are combined by ONE ``ncclAllReduce(sum, float64)`` of 32 doubles per EM
 iteration, issued by libcpd_b200.so on its own stream (cpd_comm_init / cpd_em_step).

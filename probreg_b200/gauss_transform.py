@@ -1,4 +1,4 @@
-"""Gauss transform on the B200 -- the API of ``probreg.gauss_transform`` (gauss_transform.py:28-60).
+"""Gauss transform on the H100 -- the API of ``probreg.gauss_transform`` (gauss_transform.py:28-60).
 
     sum_j weights[j] * exp(-||target[i] - source[j]||^2 / h^2)
 

@@ -1,4 +1,4 @@
-"""Caller-side helpers so that scripts written against the reference run without open3d (SURVEY section 8f, row 4):
+"""Caller-side helpers so that scripts written against the reference run without open3d:
 readers for the point-cloud files the reference ships (ASCII ``.pcd``, binary/ASCII ``.ply``, whitespace ``.txt``) and a
 voxel-grid down-sampler in the spirit of ``open3d.geometry.PointCloud.voxel_down_sample`` (per-voxel mean; the
 reference's examples/utils.py:20 and tests/test_cpd.py:12 use open3d's).  Plain numpy on the host -- this is data

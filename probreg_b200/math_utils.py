@@ -1,4 +1,4 @@
-"""The two ``probreg.math_utils`` helpers the CPD path uses, on the B200.
+"""The two ``probreg.math_utils`` helpers the CPD path uses, on the GPU.
 
 * ``squared_kernel_sum``  probreg/math_utils.py:28-29 -> ``_math.squared_kernel`` (cc/math_utils.cc:15)
 * ``rbf_kernel``          probreg/math_utils.py:36-37 -> ``_math.rbf_kernel``     (cc/math_utils.cc:17-19)

@@ -1,8 +1,8 @@
 """Synthetic workloads of BASELINE.md section 3 (used by bench.py and the examples).
 
 source = anisotropic uniform box; target = permuted, noised (sigma 0.01), transformed copy.
-An isotropic blob makes rigid CPD with update_scale collapse towards scale ~0.45 and crawl
-(SURVEY section 8d), hence the 1.0 x 0.6 x 0.3 box.
+An isotropic blob makes rigid CPD with update_scale collapse towards scale ~0.45 and crawl,
+hence the 1.0 x 0.6 x 0.3 box.
 """
 import numpy as np
 

@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE: build tests/emu/_build/libcpd_b200_emu.so, the CPU emulation of libcpd_b200.so.
 
-The product library needs a B200; the container the CPU test suite runs in has no GPU.  To still execute
+The product library needs an H100; the container the CPU test suite runs in has no GPU.  To still execute
 the library's host orchestration (csrc/cpd_b200.cu) and its kernels (csrc/kernels.cuh) there, this script
 
   1. rewrites every  `kernel<<<grid, block, smem, stream>>>(args)`  of cpd_b200.cu into

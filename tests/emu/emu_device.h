@@ -1,7 +1,7 @@
 // tests/emu/emu_device.h -- TEST INFRASTRUCTURE: host stand-ins for the inline-PTX helpers of
 // probreg_b200/csrc/kernels.cuh (included from there only when CPD_HOST_EMU is defined).
 //   ex2.approx.ftz      -> exp2f with results below FLT_MIN flushed to 0 (the property exact culling relies on)
-//   f32x2 arithmetic    -> two scalar IEEE operations per call (compile with -ffp-contract=off)
+//   FP32 pair helpers   -> two scalar IEEE operations per call (compile with -ffp-contract=off)
 //   mbarrier + TMA bulk -> the copy is performed when the barrier is waited on; until then the destination
 //                          holds a NaN pattern, so reading a stage before its wait, or re-arming a stage that
 //                          a slower thread still reads, corrupts the results visibly

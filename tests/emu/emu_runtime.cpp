@@ -242,7 +242,7 @@ struct emu_event { double t_ms; bool recorded; };
 static int emu_sms() {
     const char* e = getenv("CPD_EMU_SMS");
     const int v = e ? atoi(e) : 0;
-    return v > 0 ? v : 148;
+    return v > 0 ? v : 132;
 }
 static int emu_devices() {
     const char* e = getenv("CPD_EMU_DEVICES");
@@ -255,7 +255,7 @@ const char* cudaGetErrorString(cudaError_t e) { return e == cudaSuccess ? "no er
 cudaError_t cudaSetDevice(int d) { return (d >= 0 && d < emu_devices()) ? cudaSuccess : cudaErrorInvalidValue; }
 cudaError_t cudaGetDeviceProperties(cudaDeviceProp* p, int) {
     memset(p, 0, sizeof(*p));
-    p->major = 10; p->minor = 0; p->multiProcessorCount = emu_sms();
+    p->major = 9; p->minor = 0; p->multiProcessorCount = emu_sms();
     snprintf(p->name, sizeof(p->name), "CPU emulation (tests/emu)");
     return cudaSuccess;
 }

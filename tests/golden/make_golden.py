@@ -1,11 +1,11 @@
 #!/usr/bin/env python
 """Generate tests/golden/*.npz by running the UNMODIFIED reference (probreg v0.3.7).
 
-Runs only in the build container (``/root/reference`` must exist); the fixtures it
-writes are committed so that the GPU box, which has no reference checkout, can
+Needs a checkout of the reference named by $PROBREG_REFERENCE; the fixtures it
+writes are committed so that the tests, which never read the reference, can
 check both the oracle and the CUDA path against the reference's own outputs.
 
-How the reference is loaded (SURVEY.md section 8c): ``probreg/__init__.py`` imports
+How the reference is loaded: ``probreg/__init__.py`` imports
 every algorithm (and open3d, transforms3d, ... which are absent here), so a bare
 parent package is planted in ``sys.modules`` and only ``probreg.cpd`` /
 ``probreg.transformation`` / ``probreg.math_utils`` / ``probreg.log`` are imported,
@@ -25,7 +25,7 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-REF = os.environ.get("PROBREG_REFERENCE", "/root/reference")
+REF = os.environ.get("PROBREG_REFERENCE", "")
 sys.path.insert(0, ROOT)
 
 from oracle import cpd_oracle as orc  # noqa: E402
@@ -85,7 +85,7 @@ def main():
     rz = orc.rot_z(30.0)
     bunny_t = bunny.dot(rz.T)
 
-    # ---- 1. bunny: init, first E-step, rigid/affine registrations (SURVEY appendix C)
+    # ---- 1. bunny: init, first E-step, rigid/affine registrations
     g = {"source": bunny, "target": bunny_t}
     r = cpd.RigidCPD(bunny)
     ini = r._initialize(bunny_t)
@@ -123,7 +123,7 @@ def main():
     for seed in range(7, 100):
         # far outliers whose nearest-source exponent stays clear of float64's denormal band
         # (-708 .. -745.13): there the reference's own K values carry only a few bits, so no
-        # implementation can be compared against it element-wise (SURVEY section 7, hard part 3)
+        # implementation can be compared against it element-wise
         rng = np.random.default_rng(seed)
         outl = (rng.random((200, 3)) - 0.5) * 3.0 + tgt.mean(0)
         d2min = ((ts_true[:, None, :] - outl[None, :, :]) ** 2).sum(-1).min(0)

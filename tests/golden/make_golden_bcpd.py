@@ -2,8 +2,12 @@
 """Generate tests/golden/bcpd.npz by running the UNMODIFIED reference probreg/bcpd.py (v0.3.7).
 
 Same loading trick as make_golden.py (a bare parent package, open3d stubbed, probreg._math replaced by float32 numpy
-restatements) plus ``_math.inverse_multiquadric_kernel`` restated from cc/math_utils.cc:37-39 in float32.  Runs only in
-the build container; the .npz is committed.   Usage:  python tests/golden/make_golden_bcpd.py
+restatements) plus ``_math.inverse_multiquadric_kernel`` restated from cc/math_utils.cc:37-39 in float32.  Needs a checkout of
+the reference named by $PROBREG_REFERENCE; the files it writes are committed.   Usage:  python tests/golden/make_golden_bcpd.py
+
+Besides bcpd.npz it writes bcpd_reg_gmat_inv.npy: the float32 inverse of the registration's kernel matrix exactly as the
+reference computes it (np.linalg.inv in CombinedBCPD._initialize) on THIS host.  That inverse (condition ~1e10) depends on the
+host's LAPACK build, and the registration fixture depends on it; the tests replay it so that the fixture holds on any host.
 """
 import importlib
 import os
@@ -60,7 +64,8 @@ def main():
     out["reg_source"], out["reg_target"] = s_small, t_small
     out["reg_rot"], out["reg_t"], out["reg_scale"], out["reg_v"] = tfm.rigid_trans.rot, tfm.rigid_trans.t, tfm.rigid_trans.scale, tfm.v
     np.savez_compressed(os.path.join(HERE, "bcpd.npz"), **out)
-    print("wrote bcpd.npz")
+    np.save(os.path.join(HERE, "bcpd_reg_gmat_inv.npy"), reg.gmat_inv)
+    print("wrote bcpd.npz, bcpd_reg_gmat_inv.npy")
 
 
 if __name__ == "__main__":

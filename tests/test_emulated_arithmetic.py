@@ -1,4 +1,4 @@
-"""CPU evidence for the precision design (DESIGN.md section 2): the arithmetic the CUDA kernels perform -- FP32 pair maths
+"""CPU evidence for the precision design: the arithmetic the CUDA kernels perform -- FP32 pair maths
 with the same FMA chains, integer offsets, two-level FP32 group sums, FP64 beyond, residual-form M-step -- emulated in
 numpy (tools/emulate_resid.py, exactly rounded exp2 instead of MUFU.EX2) meets the north-star tolerances against the
 fixtures produced by the reference.  The GPU tests check the real kernels; this one runs without a GPU."""

@@ -111,7 +111,7 @@ def test_multi_wave_work_lists_under_emulation(emulated, monkeypatch, sms):
 
 @pytest.mark.parametrize("unit,last_cost", [("stage", "1.0"), ("subchunk", "1.0"), ("subchunk", "0.3"), ("stage", "0.6")])
 def test_pass1_plan_switches_under_emulation(emulated, monkeypatch, unit, last_cost):
-    """Pass 1's work plan (tuning switches of DESIGN section 4): whole stages or sub-chunks as the unit of the cuts, any cost of the
+    """Pass 1's work plan (tuning switches): whole stages or sub-chunks as the unit of the cuts, any cost of the
     last tile -- items that begin and end inside a TMA stage, a last tile whose warps of padding leave the kernel at once (1300
     targets: 276 in the second tile, 3 of its 8 warps alive).  The plan must never show in the results."""
     from oracle import cpd_oracle as orc
@@ -148,7 +148,7 @@ def test_results_do_not_depend_on_the_thread_schedule(emu_lib_path):
 def test_parity_survives_a_mufu_like_ex2(emu_lib_path):
     """Re-run a slice of the emulated tests with ex2 perturbed by up to 2^-22 relative, smoothly in the fractional part of its
     argument (CPD_EMU_EX2=mufu): parity must not hinge on an exact exp2 -- the two passes see identical arguments, so the error
-    cancels in K / sum K (DESIGN section 2, decision 2; section 4d for the weighted instantiations)."""
+    cancels in K / sum K."""
     import os
     import subprocess
     import sys

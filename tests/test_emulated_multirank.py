@@ -1,4 +1,4 @@
-"""The target-sharded multi-rank path (SURVEY section 8e) on the CPU: ranks are threads, each with its own handle and "device" of
+"""The target-sharded multi-rank path on the CPU: ranks are threads, each with its own handle and "device" of
 the emulated library (tests/emu), and ncclAllReduce is an in-process rendezvous (tests/emu/emu_nccl.h).  What runs for real: the
 shard bounds / global N / common frame origin, the per-shard E-step, the moments all-reduce + replicated M-step of the rigid and
 affine loops, the M-sized all-reduces of cpd_estep, the non-rigid (dense, low-rank, constrained) paths -- compared with the

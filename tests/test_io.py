@@ -1,4 +1,5 @@
-"""probreg_b200.io: readers and the voxel down-sampler (CPU; the optional part uses the reference's data when present)."""
+"""probreg_b200.io: readers and the voxel down-sampler (CPU), on synthetic files and on data files of the reference project stored
+under tests/golden/data (bunny.pcd and the fish clouds whole; horse.ply and cloud_0.pcd cut to their first vertices)."""
 import os
 import struct
 
@@ -7,7 +8,7 @@ import pytest
 
 from probreg_b200 import io as pio
 
-REF = "/root/reference"
+DATA = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "data")
 
 
 def test_pcd_and_txt_roundtrip(tmp_path):
@@ -48,16 +49,24 @@ def test_voxel_down_sample():
         pio.voxel_down_sample(cloud, 0.0)
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference checkout not present")
 def test_reference_fixtures_load():
-    bunny = pio.read_points(os.path.join(REF, "examples", "bunny.pcd"))
+    bunny = pio.read_points(os.path.join(DATA, "bunny.pcd"))
     assert bunny.shape == (397, 3)                                            # examples/bunny.pcd:9
-    assert abs(pio.voxel_down_sample(bunny, 0.005).shape[0] - 381) <= 12      # SURVEY: ~381 points at voxel 0.005
-    horse = pio.read_points(os.path.join(REF, "data", "horse.ply"))
-    assert horse.shape == (48485, 3)                                          # binary_big_endian, 48 485 vertices
-    assert abs(pio.voxel_down_sample(horse, 0.01).shape[0] - 480) <= 40       # tests/test_cpd.py recipe: ~480 points
-    assert pio.read_points(os.path.join(REF, "examples", "cloud_0.pcd")).shape == (6535, 3)
-    assert pio.read_points(os.path.join(REF, "examples", "fish_source.txt")).shape == (91, 2)
+    assert abs(pio.voxel_down_sample(bunny, 0.005).shape[0] - 381) <= 12      # the reference's recipe: ~381 points at voxel 0.005
+    # data/horse.ply: binary_big_endian, x y z confidence r g b per vertex, then a face list; here the first 2000 of its 48 485
+    # vertices and its first 10 faces (the full file gives 487 voxels at 0.01, the tests/test_cpd.py recipe's ~480)
+    path = os.path.join(DATA, "horse_head.ply")
+    horse = pio.read_points(path)
+    assert horse.shape == (2000, 3)
+    raw = open(path, "rb").read()
+    body = raw[raw.index(b"end_header\n") + len(b"end_header\n"):]
+    rec = np.frombuffer(body[: 2000 * 19], dtype=np.dtype([("xyz", ">f4", 3), ("c", ">f4"), ("rgb", "u1", 3)]))
+    np.testing.assert_array_equal(horse, rec["xyz"].astype(np.float64))
+    assert pio.voxel_down_sample(horse, 0.01).shape[0] == 32
+    cloud = pio.read_points(os.path.join(DATA, "cloud_0_head.pcd"))          # first 300 of 6535 points, 8 fields each
+    assert cloud.shape == (300, 3)
+    np.testing.assert_allclose(cloud[0], [0.67162704, 0.36310977, 1.4365245], rtol=1e-7)
+    assert pio.read_points(os.path.join(DATA, "fish_source.txt")).shape == (91, 2)
 
 
 def test_example_utils_follow_the_reference_recipes():
@@ -74,16 +83,14 @@ def test_example_utils_follow_the_reference_recipes():
     r = ex.euler2mat(0.1, -0.2, 0.3)
     np.testing.assert_allclose(r.dot(r.T), np.identity(3), atol=1e-15)
     np.testing.assert_allclose(ex.euler2mat(0.0, 0.0, np.deg2rad(30.0))[:2, :2], [[np.cos(np.pi / 6), -0.5], [0.5, np.cos(np.pi / 6)]], atol=1e-15)
-    bunny = ex.reference_file("bunny.pcd")
-    if bunny is None:
-        return                                                          # the reference's data files are not around (GPU box)
+    bunny = os.path.join(DATA, "bunny.pcd")
     src, tgt = ex.prepare_source_and_target_rigid_3d(bunny, rng=np.random.default_rng(0))
     assert src.shape[1] == 3 and tgt.shape == (src.shape[0] + 500, 3)
     # undo the known transform: the inliers are the (shuffled, slightly noised) source
     back = tgt[: src.shape[0]].dot(ex.euler2mat(0.0, 0.0, np.deg2rad(30.0)))
     d = np.sqrt(((back[:, None, :] - src[None, :, :]) ** 2).sum(-1)).min(axis=1)
     assert d.max() < 0.01
-    fish = ex.prepare_source_and_target_nonrigid_2d(ex.reference_file("fish_source.txt"), ex.reference_file("fish_target.txt"))
+    fish = ex.prepare_source_and_target_nonrigid_2d(os.path.join(DATA, "fish_source.txt"), os.path.join(DATA, "fish_target.txt"))
     assert fish[0].shape == (91, 2) and fish[1].shape == (91, 2)
 
 

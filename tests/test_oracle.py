@@ -28,7 +28,7 @@ def test_rbf_symmetric_and_golden():
 def test_init_matches_reference(bunny):
     s2 = orc.sigma2_init(bunny["source"], bunny["target"])
     assert s2 == float(bunny["init_sigma2"])            # float32 value, bit-exact
-    assert s2 == pytest.approx(0.0036908406764268875, rel=1e-12)   # SURVEY appendix C
+    assert s2 == pytest.approx(0.0036908406764268875, rel=1e-12)   # the reference's value
     assert orc.sigma2_init_exact(bunny["source"], bunny["target"]) == pytest.approx(s2, rel=2e-7)
     q0 = 1.0 + bunny["target"].shape[0] * 3 * 0.5 * np.log(np.float32(s2))
     assert float(q0) == pytest.approx(float(bunny["init_q"]), rel=1e-12)
@@ -115,7 +115,7 @@ def test_default_tolerance_iteration_count(bunny, tag, tf_type):
 
 
 def test_appendix_c_values(bunny):
-    # SURVEY.md appendix C, regenerated here by the reference itself
+    # values regenerated by the reference itself (tests/golden/make_golden.py)
     assert int(bunny["rigid_default_iters"]) == 18
     assert float(bunny["rigid_default_sigma2"]) == pytest.approx(1.1920928955078125e-07)
     assert float(bunny["rigid10_sigma2"]) == pytest.approx(3.9235098811641994e-05, rel=1e-9)

@@ -1,8 +1,8 @@
 """BASELINE.json configurations 3 and 4 at full size through size-independent properties (no oracle can hold them):
    3. affine CPD, N = M = 250k on one GPU;   4. rigid CPD, N = M = 1M sharded over 8 GPUs -> here ONE rank's shard
    (1M sources x 125k targets, the global N in the outlier constant), which is what each of the 8 processes executes.
-First hardware run: round 2.  Config 3 needs ~300 iterations at 250k, not the ~100 of a 3000-point cloud: EM anneals sigma2 more
-slowly the denser the cloud is (measured on the B200, profiles/r2_convergence_traces.txt: 3k points converge by iteration 75,
+Config 3 needs ~300 iterations at 250k, not the ~100 of a 3000-point cloud: EM anneals sigma2 more
+slowly the denser the cloud is (3k points converge by iteration 75,
 30k by 175, 250k by ~350; the 3k trajectory is the oracle's).
 """
 import numpy as np
@@ -51,7 +51,7 @@ def _config4(m, n_global, ranks, sample):
 @pytest.mark.gpu
 @pytest.mark.timeout(900)
 def test_config3_affine_250k_properties():
-    _config3(250000, 300, 600)           # |B - B*| 3.0e-3, sigma2 1.03e-4 after 300 iterations (profiles/r2_convergence_traces.txt)
+    _config3(250000, 300, 600)           # |B - B*| 3.0e-3, sigma2 1.03e-4 after 300 iterations
 
 
 @pytest.mark.gpu

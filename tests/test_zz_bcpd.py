@@ -1,11 +1,9 @@
-"""BCPD E-step on the pair kernels (SURVEY section 8(f) row 3) and the ``probreg.bcpd`` surface around it.
+"""BCPD E-step on the pair kernels and the ``probreg.bcpd`` surface around it.
 
 Fixtures: tests/golden/bcpd.npz, produced by the UNMODIFIED reference bcpd.py (tests/golden/make_golden_bcpd.py).
 CPU tests: the oracle against those fixtures, and the library under the emulation of tests/emu; the gpu-marked tests run the same
-bodies on the B200 (first hardware run: round 2, profiles/r2_pytest_runxfail_first.txt).
+bodies on the GPU.
 """
-import os
-
 import numpy as np
 import pytest
 
@@ -113,32 +111,28 @@ def _run_registration(g):
 
 
 def _check_registration_vs_fixture():
-    """Against the committed outputs of the reference.  Only meaningful on the host (CPU + numpy/LAPACK build) that generated the
-    fixture: the reference's own M-step calls np.linalg.inv on a float32 matrix of condition 1.3e10, whose result differs between
-    LAPACK kernels.  The CPU suite runs where the fixture was made; the GPU box uses _check_registration_vs_reference_here."""
+    """Against the committed outputs of the unmodified reference bcpd.py (five iterations on the same inputs).  The reference's own
+    M-step calls np.linalg.inv on a float32 matrix of condition 1.3e10, so its result depends on the host's LAPACK build; what this
+    package computes itself -- the kernel matrix (bit-exact) and five E-steps -- is what the tolerance below judges.  So that the
+    comparison holds on any host, that one inverse is the fixture host's (bcpd_reg_gmat_inv.npy, computed where the fixture was
+    made): np.linalg.inv returns it for exactly that matrix."""
     g = load_golden("bcpd.npz")
-    tfm = _run_registration(g)
+    gmat = orc.imq_kernel_f32(g["reg_source"], g["reg_source"], 1.0)
+    gmat_inv = load_golden("bcpd_reg_gmat_inv.npy")
+    inv = np.linalg.inv
+
+    def fixture_host_inv(a):
+        return gmat_inv.copy() if (a.dtype == np.float32 and np.array_equal(a, gmat)) else inv(a)
+
+    np.linalg.inv = fixture_host_inv
+    try:
+        tfm = _run_registration(g)
+    finally:
+        np.linalg.inv = inv
     np.testing.assert_allclose(tfm.rigid_trans.rot, g["reg_rot"], atol=1e-5)
     np.testing.assert_allclose(tfm.rigid_trans.t, g["reg_t"], atol=1e-5)
     assert tfm.rigid_trans.scale == pytest.approx(float(g["reg_scale"]), rel=1e-5)
     np.testing.assert_allclose(tfm.v, g["reg_v"], atol=1e-5)
-
-
-def _check_registration_vs_reference_here():
-    """registration_bcpd against the UNMODIFIED reference bcpd.py (baseline/_ref, see baseline/install_ref.py) run on THIS host
-    with the same inputs: both sides then invert the same float32 kernel matrix with the same LAPACK, and what is compared is
-    what this package computes itself -- the kernel matrix (bit-exact) and five E-steps on the GPU."""
-    from baseline import ref_loader
-    if not ref_loader.available() or not os.path.isfile(os.path.join(ref_loader.REF_DIR, "bcpd.py")):
-        pytest.skip("baseline/_ref/probreg/bcpd.py is missing (python baseline/install_ref.py where /root/reference exists)")
-    rb = ref_loader.load_bcpd()
-    g = load_golden("bcpd.npz")
-    ref = rb.CombinedBCPD(g["reg_source"], lmd=2.0).registration(g["reg_target"], w=0.05, maxiter=5, tol=-1.0)
-    tfm = _run_registration(g)
-    np.testing.assert_allclose(tfm.rigid_trans.rot, ref.rigid_trans.rot, atol=1e-5)
-    np.testing.assert_allclose(tfm.rigid_trans.t, ref.rigid_trans.t, atol=1e-5)
-    assert tfm.rigid_trans.scale == pytest.approx(float(ref.rigid_trans.scale), rel=1e-5)
-    np.testing.assert_allclose(tfm.v, ref.v, atol=1e-5)
 
 
 @pytest.mark.parametrize("tag", CASES)
@@ -153,7 +147,6 @@ def test_bcpd_estep_shapes_emulated(emulated):
 def test_bcpd_registration_emulated(emulated):
     _check_imq_kernel()
     _check_registration_vs_fixture()
-    _check_registration_vs_reference_here()
 
 
 def test_bcpd_culled_estep_is_bit_exact_emulated(emulated, monkeypatch):
@@ -188,10 +181,25 @@ def test_bcpd_estep_shapes_gpu():
 
 
 @pytest.mark.gpu
-@pytest.mark.timeout(600)
-def test_bcpd_registration_gpu():
+@pytest.mark.timeout(900)
+def test_bcpd_registration_gpu(emu_lib_path):
+    """Five iterations on the GPU against the committed outputs of the unmodified reference (with the fixture host's inverse
+    replayed, see _check_registration_vs_fixture), and -- with this host's own LAPACK on both sides -- against the CPU emulation
+    of the same sources."""
     _check_imq_kernel()
-    _check_registration_vs_reference_here()
+    _check_registration_vs_fixture()
+    g = load_golden("bcpd.npz")
+    tfm = _run_registration(g)
+    saved = _cabi._lib
+    _cabi._lib = _cabi._load(emu_lib_path)
+    try:
+        ref = _run_registration(g)
+    finally:
+        _cabi._lib = saved
+    np.testing.assert_allclose(tfm.rigid_trans.rot, ref.rigid_trans.rot, atol=1e-5)
+    np.testing.assert_allclose(tfm.rigid_trans.t, ref.rigid_trans.t, atol=1e-5)
+    assert tfm.rigid_trans.scale == pytest.approx(float(ref.rigid_trans.scale), rel=1e-5)
+    np.testing.assert_allclose(tfm.v, ref.v, atol=1e-5)
 
 
 def _check_full_size(n, sample):

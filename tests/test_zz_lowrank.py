@@ -1,12 +1,11 @@
-"""Low-rank non-rigid CPD (BASELINE configuration 5, SURVEY section 8(f) row 1) and the device-side correspondence priors.
+"""Low-rank non-rigid CPD (BASELINE configuration 5) and the device-side correspondence priors.
 
 There is no reference counterpart for the low-rank path (the reference solves the dense M x M system, cpd.py:296), so
-parity is anchored as SURVEY section 8(f) says: against the reference's dense arithmetic (the numpy oracle) at sizes where the
+parity is anchored against the reference's dense arithmetic (the numpy oracle) at sizes where the
 dense solve is possible, with the truncation error of the factorisation as the tolerance, and -- tighter -- against the
 oracle run on the SAME approximate G = Q Bc Q^T, where only rounding separates the two.
 
-CPU tests run the library under the emulation of tests/emu; the gpu-marked ones call the real library (first hardware run: round 2,
-profiles/r2_pytest_runxfail_first.txt -- the one failure there was the iteration count of the config-5 property test, see below).
+CPU tests run the library under the emulation of tests/emu; the gpu-marked ones call the real library.
 """
 import os
 
@@ -415,8 +414,8 @@ def test_config5_body_at_emulation_size(emulated):
 @pytest.mark.gpu
 @pytest.mark.timeout(600)
 def test_lowrank_baseline_config5_properties():
-    _check_config5(6000, 50000, 200, 80)      # residual 0.26 of the applied deformation after 80 iterations (0.43 after 60:
-                                                # profiles/r2_convergence_traces.txt; the dense loop at 12k follows the same curve)
+    _check_config5(6000, 50000, 200, 80)      # residual 0.26 of the applied deformation after 80 iterations (0.43 after 60;
+                                                # the dense loop at 12k follows the same curve)
 
 
 _PRODUCT_SCRIPT = r"""
@@ -437,11 +436,9 @@ np.save(sys.argv[1], q.dot(b).dot(q.T))
 @pytest.mark.gpu
 @pytest.mark.timeout(900)
 def test_every_selectable_gram_product_gives_the_same_factorisation(tmp_path):
-    """CPD_B200_LR_GRAM selects the kernel behind the G X products of the range finder: the exact integer-digit tensor-core kernels
-    (A operand in tensor memory -- the default -- or in shared memory), the TF32 x 3 tensor-core kernel, the CUDA-core kernel.  The
-    variable is read once per process, hence subprocesses.  The two integer kernels and the CUDA-core kernel agree with the float32
-    G of the reference to 1e-6 (relative, spectral norm); the TF32 kernel to the 3e-5 its truncating FP32 accumulation in TMEM
-    allows (DESIGN 4c) -- which is why it is not the default.  A rank of 130 takes two column passes, 1300 points 11 row tiles."""
+    """CPD_B200_LR_GRAM selects the kernel behind the G X products of the range finder: the exact integer-digit tensor-core kernel
+    (the default) or the CUDA-core kernel.  The variable is read once per process, hence subprocesses.  Both agree with the float32
+    G of the reference to 1e-6 (relative, spectral norm).  A rank of 130 takes three column passes, 1300 points 11 row tiles."""
     import subprocess
     import sys
 
@@ -452,11 +449,10 @@ def test_every_selectable_gram_product_gives_the_same_factorisation(tmp_path):
     g = orc.rbf_kernel_f32(src, src, beta).astype(np.float64)
     code = _PRODUCT_SCRIPT % (ROOT, m, beta, rank)
     errs = {}
-    for mode in ("i8", "i8ss", "simt", "tf32"):
+    for mode in ("i8", "simt"):
         out = str(tmp_path / ("g_%s.npy" % mode))
         r = subprocess.run([sys.executable, "-c", code, out], capture_output=True, text=True, timeout=600,
                            env=dict(os.environ, CPD_B200_LR_GRAM=mode))
         assert r.returncode == 0, (mode, r.stderr[-2000:])
         errs[mode] = np.linalg.norm(np.load(out) - g, 2) / np.linalg.norm(g, 2)
-    assert errs["i8"] < 1e-6 and errs["i8ss"] < 1e-6 and errs["simt"] < 1e-6, errs
-    assert errs["tf32"] < 3e-5, errs
+    assert errs["i8"] < 1e-6 and errs["simt"] < 1e-6, errs

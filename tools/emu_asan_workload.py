@@ -1,4 +1,4 @@
-"""AddressSanitizer sweep of the emulated library (test infrastructure; see DESIGN.md section 8).
+"""AddressSanitizer sweep of the emulated library (test infrastructure; see tests/emu/README.md).
 
 Build:  g++ -O1 -g -std=c++17 -fPIC -shared -ffp-contract=off -fno-strict-aliasing -w -fsanitize=address -fno-omit-frame-pointer -DEMU_UCONTEXT \
         -Itests/emu -Itests/emu/_build -Iinclude -Iprobreg_b200/csrc -o tests/emu/_build/libcpd_b200_emu_asan.so \

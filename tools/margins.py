@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Measured parity margins on the GPU (what the tolerances of tests/ leave unused): prints max deviations, asserts nothing.
-   usage: python tools/margins.py > profiles/r2_parity_margins.txt   (needs tests/golden/*.npz; the oracle is the checker)"""
+   usage: python tools/margins.py   (needs tests/golden/*.npz; the oracle is the checker)"""
 import os, sys
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

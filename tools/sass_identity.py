@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Per-kernel comparison of the SASS of two builds of libcpd_b200.so (cuobjdump -sass, addresses stripped): which kernels are
 byte-identical, which changed, which are new.  The check that a refactor or a new template parameter left the measured kernels
-alone (profiles/r1_sass_identity.txt).   usage: sass_identity.py old.so new.so [--fold 'ILb0ELb0EEE=ILb0EEE' ...]"""
+alone.   usage: sass_identity.py old.so new.so [--fold 'ILb0ELb0EEE=ILb0EEE' ...]"""
 import hashlib
 import re
 import subprocess
