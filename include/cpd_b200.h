@@ -128,6 +128,14 @@ int cpd_nonrigid_mstep(cpd_ctx* h, const double* pt1, const double* p1, const do
  * the default form: positive semi-definite, exactly the core the iteration uses); any may be NULL. */
 int cpd_nonrigid_lowrank_begin(cpd_ctx* h, double beta, double lmd, double sigma2, double w, int rank, int power_iters, uint64_t seed);
 int cpd_nonrigid_lowrank_get(cpd_ctx* h, int* rank_out, double* q_out, double* bcore_out);
+/* Test / diagnostic entry (like cpd_plan_work): out = G x for the G of the last cpd_nonrigid_lowrank_begin on this handle (its beta
+ * and source points; the source must not have changed since).  x and out are m x cols (1 <= cols <= 1024), row-major, in the
+ * caller's point order.  kernel 0: the exact integer-digit product on the tensor cores (csrc/gram_i8.cuh), 1: the CUDA-core kernel
+ * (csrc/lowrank.cuh); the call goes straight to it, without the first-use self-check.  world = 1, rank = 0: every row; otherwise
+ * only the rows that rank `rank` of a `world`-rank handle forms are filled and the others are zero (there is no exchange).  The
+ * factors and the iteration state are left as they were.  The CPU emulation of the test-suite has no tensor-core product: kernel 0
+ * fails there with CPD_ERR_STATE. */
+int cpd_lowrank_gram_product(cpd_ctx* h, const double* x, int cols, int kernel, int world, int rank, double* out);
 
 /* Another registration with the same source (one template, many targets): resets W = 0 (cpd.py:281), the moved source, sigma2, w,
  * lmd and the priors, and keeps G / the low-rank factors of the last cpd_nonrigid_*begin.  The caller vouches that the source

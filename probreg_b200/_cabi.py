@@ -51,6 +51,7 @@ _PROTOS = {
     "cpd_nonrigid_lowrank_begin": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_double, ctypes.c_double, ctypes.c_double, ctypes.c_double,
                                                   ctypes.c_int, ctypes.c_int, ctypes.c_uint64]),
     "cpd_nonrigid_lowrank_get": (ctypes.c_int, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_int), _c_dp, _c_dp]),
+    "cpd_lowrank_gram_product": (ctypes.c_int, [ctypes.c_void_p, _c_dp, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_dp]),
     "cpd_nonrigid_set_prior": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_double, _c_dp, _c_dp]),
     "cpd_rbf_kernel": (ctypes.c_int, [ctypes.c_int, _c_dp, ctypes.c_int64, _c_dp, ctypes.c_int64, ctypes.c_int,
                                       ctypes.c_double, _c_fp]),
@@ -262,6 +263,18 @@ class Handle(object):
         q, b = np.empty((self.m, k.value)), np.empty((k.value, k.value))
         check(self._lib.cpd_nonrigid_lowrank_get(self._h, None, dptr(q), dptr(b)))
         return q, b
+
+    GRAM_TENSOR_CORES, GRAM_CUDA_CORES = 0, 1
+
+    def lowrank_gram_product(self, x, kernel, world=1, rank=0):
+        """G x (m x cols) for the G of the last nonrigid_lowrank_begin, by one kernel (GRAM_TENSOR_CORES or GRAM_CUDA_CORES);
+        with world > 1 only the rows of `rank`'s share are filled.  A test / diagnostic entry: the factors stay as they were."""
+        xa = np.ascontiguousarray(x, dtype=np.float64)
+        if xa.ndim != 2 or xa.shape[0] != self.m:
+            raise ValueError("x must be m x cols with m = %d, got %s" % (self.m, xa.shape))
+        out = np.empty_like(xa)
+        check(self._lib.cpd_lowrank_gram_product(self._h, dptr(xa), xa.shape[1], int(kernel), int(world), int(rank), dptr(out)))
+        return out
 
     def nonrigid_set_prior(self, alpha, p1_tilde, px_tilde):
         if p1_tilde is None:

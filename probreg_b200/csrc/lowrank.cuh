@@ -819,5 +819,14 @@ lr_export_kernel(const double* __restrict__ Q, const int* __restrict__ perm, lon
         for (int k = 0; k < rank; ++k) out[r * rank + k] = Q[(long long)k * ld + i];
     }
 }
+// X[k][i] = in[perm[i]][k]: the inverse of lr_export_kernel (a row-major M x K block in the caller's order -> [K][ld], internal order)
+__global__ void __launch_bounds__(THREADS)
+lr_import_kernel(const double* __restrict__ in, const int* __restrict__ perm, long long m, long long ld, int rank, double* __restrict__ X) {
+    const long long i = (long long)blockIdx.x * THREADS + threadIdx.x;
+    if (i < m) {
+        const long long r = perm[i];
+        for (int k = 0; k < rank; ++k) X[(long long)k * ld + i] = in[r * rank + k];
+    }
+}
 
 }  // namespace cpd
