@@ -102,6 +102,24 @@ int cpd_mstep(cpd_ctx* h, int tf_kind, int update_scale, const double* pt1, cons
 int cpd_bcpd_estep(cpd_ctx* h, const double* t_source, double scale, const double* alpha, const double* sigma_diag, double sigma2,
                    double w, double* nu_d, double* nu, double* px, double* n_p);
 
+/* CombinedBCPD.registration (probreg/bcpd.py:82-156) resident on the device, after cpd_set_source / cpd_set_target.
+ * gmat_inv: the caller's m x m float32 inverse of the IMQ kernel matrix (row-major, caller's point order; bcpd.py:113-114).  It is
+ * uploaded once and kept in float32; the handle holds it, the FP64 precision matrix A and the posterior covariance Sigma: about
+ * 20 m^2 bytes (8 GB at m = 20k).  lmd, k > 0, sigma2 > 0, 0 <= w < 1.
+ * Starts from the reference's _initialize: identity similarity, v = 0, alpha = 1/m, diag(sigma_mat) = 1, the given sigma2.
+ * Refused (CPD_ERR_STATE) on a handle with a communicator attached: the loop runs on one GPU.                               */
+int cpd_bcpd_begin(cpd_ctx* h, const float* gmat_inv, double lmd, double k, double sigma2, double w);
+/* One loop body: E-step on T(y) = s R (y + v) + t, then the M-step of bcpd.py:125-156 (Sigma = A^-1 by cuSOLVER's LU and a solve
+ * against the identity; v = ratio Sigma r without a division by nu, so a source no target explains keeps v finite).
+ * *sigma2_out: the new sigma2.  The target may be set again between two steps (any count); the loop goes on from its state.
+ * Fails with CPD_ERR_STATE before cpd_bcpd_begin, after the source was set again, when getrf finds U exactly singular or getrs
+ * fails, or when the new sigma2 is not a positive finite number; after such a failure every step fails until the next
+ * cpd_bcpd_begin.                                                                                                               */
+int cpd_bcpd_step(cpd_ctx* h, double* sigma2_out);
+/* The current state, caller's order; any pointer may be NULL.  sim: lin = rot, t, scale, sigma2 (n_p: of the last E-step).
+ * v_out, moved_out (s R (y + v) + t): m x D;  alpha_out, sigma_diag_out: m.                                                    */
+int cpd_bcpd_get(cpd_ctx* h, cpd_params* sim, double* v_out, double* moved_out, double* alpha_out, double* sigma_diag_out);
+
 /* Copies of the last E-step's reductions (device -> host), valid after cpd_em_step/run. */
 int cpd_last_estep(cpd_ctx* h, double* pt1, double* p1, double* px, double* n_p);
 
@@ -201,6 +219,9 @@ int cpd_event_elapsed(cpd_ctx* h, int idx_start, int idx_stop, float* ms);
  * [0] pack [1] pass1 [2] finalize1 [3] pass2 [4] finalize2 [5] moments+mstep (+allreduce)  */
 int cpd_set_profiling(cpd_ctx* h, int on);
 int cpd_stage_times(cpd_ctx* h, float ms[6]);
+/* the last cpd_bcpd_step run with profiling on, ms: [0] E-step [1] building the precision matrix [2] getrf [3] getrs against the
+ * identity [4] the rest of the M-step                                                                                          */
+int cpd_bcpd_step_times(cpd_ctx* h, float ms[5]);
 /* the last cpd_nonrigid_lowrank_begin run with profiling on: ms of [0] the G X products [1] the orthonormalisations [2] Bc       */
 int cpd_lowrank_setup_times(cpd_ctx* h, float ms[3]);
 /* launches issued by this handle since creation (kernels only).                         */

@@ -43,6 +43,10 @@ _PROTOS = {
     "cpd_bcpd_estep": (ctypes.c_int, [ctypes.c_void_p, _c_dp, ctypes.c_double, _c_dp, _c_dp, ctypes.c_double, ctypes.c_double,
                                       _c_dp, _c_dp, _c_dp, _c_dp]),
     "cpd_last_estep": (ctypes.c_int, [ctypes.c_void_p, _c_dp, _c_dp, _c_dp, _c_dp]),
+    "cpd_bcpd_begin": (ctypes.c_int, [ctypes.c_void_p, _c_fp, ctypes.c_double, ctypes.c_double, ctypes.c_double, ctypes.c_double]),
+    "cpd_bcpd_step": (ctypes.c_int, [ctypes.c_void_p, _c_dp]),
+    "cpd_bcpd_get": (ctypes.c_int, [ctypes.c_void_p, ctypes.POINTER(CpdParams), _c_dp, _c_dp, _c_dp, _c_dp]),
+    "cpd_bcpd_step_times": (ctypes.c_int, [ctypes.c_void_p, _c_fp]),
     "cpd_nonrigid_begin": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_double, ctypes.c_double, ctypes.c_double, ctypes.c_double]),
     "cpd_nonrigid_step": (ctypes.c_int, [ctypes.c_void_p, _c_dp]),
     "cpd_nonrigid_get": (ctypes.c_int, [ctypes.c_void_p, _c_dp, _c_dp]),
@@ -230,6 +234,41 @@ class Handle(object):
         check(self._lib.cpd_bcpd_estep(self._h, dptr(ts), float(scale), dptr(al), dptr(sd), float(sigma2), float(w), dptr(nu_d), dptr(nu),
                                    dptr(px), ctypes.byref(n_p)))
         return nu_d, nu, px, n_p.value
+
+    # -- BCPD registration loop (G^-1, A and Sigma resident on the device)
+    def bcpd_begin(self, gmat_inv, lmd, k, sigma2, w):
+        """Start CombinedBCPD's loop from the reference's _initialize; gmat_inv: the (m, m) C-contiguous float32 inverse of the
+        kernel matrix, in the caller's point order (set_source / set_target first)."""
+        if not isinstance(gmat_inv, np.ndarray) or gmat_inv.dtype != np.float32:
+            raise ValueError("gmat_inv must be a float32 numpy array, got %s" % getattr(gmat_inv, "dtype", type(gmat_inv)))
+        if gmat_inv.shape != (self.m, self.m):
+            raise ValueError("gmat_inv must be %d x %d (the handle's source count), got %s" % (self.m, self.m, gmat_inv.shape))
+        if not gmat_inv.flags["C_CONTIGUOUS"]:
+            raise ValueError("gmat_inv must be C-contiguous (row-major)")
+        check(self._lib.cpd_bcpd_begin(self._h, gmat_inv.ctypes.data_as(_c_fp), float(lmd), float(k), float(sigma2), float(w)))
+
+    def bcpd_step(self):
+        """One iteration; returns the new sigma2."""
+        out = ctypes.c_double()
+        check(self._lib.cpd_bcpd_step(self._h, ctypes.byref(out)))
+        return out.value
+
+    def bcpd_get(self, v=True, moved=False, alpha=False, sigma_diag=False):
+        """(rot, t, scale, sigma2, v, moved, alpha, sigma_diag) of the loop's current state in the caller's order; the arrays not
+        asked for are None."""
+        p = CpdParams()
+        va = np.empty((self.m, self.dim)) if v else None
+        mv = np.empty((self.m, self.dim)) if moved else None
+        al = np.empty(self.m) if alpha else None
+        sd = np.empty(self.m) if sigma_diag else None
+        check(self._lib.cpd_bcpd_get(self._h, ctypes.byref(p), dptr(va), dptr(mv), dptr(al), dptr(sd)))
+        rot, t, scale, sigma2 = self._unpack(p)[:4]
+        return rot, t, scale, sigma2, va, mv, al, sd
+
+    def bcpd_step_times(self):
+        ms = (ctypes.c_float * 5)()
+        check(self._lib.cpd_bcpd_step_times(self._h, ms))
+        return {"estep_ms": ms[0], "system_ms": ms[1], "getrf_ms": ms[2], "getrs_ms": ms[3], "rest_ms": ms[4]}
 
     def last_estep(self):
         pt1, p1, px = np.empty(self.n), np.empty(self.m), np.empty((self.m, self.dim))

@@ -1,11 +1,12 @@
-"""Bayesian Coherent Point Drift -- the API surface of ``probreg.bcpd`` with the E-step on the H100.
+"""Bayesian Coherent Point Drift -- the API surface of ``probreg.bcpd`` with the registration loop on the H100.
 
-What is accelerated is ``BayesianCoherentPointDrift.expectation_step`` (reference: bcpd.py:53-72): it is
-the CPD E-step with one weight per source point and runs in the same two sm_90a passes (``cpd_bcpd_estep``, the ``WGT``
-instantiations of the pair kernels), so the M x N matrix the reference materialises never exists.  The M-step of ``CombinedBCPD``
-(reference: bcpd.py:127-156) is dense M x M linear algebra that the reference itself performs on the host -- two matrix inverses per
-iteration -- and is outside the accelerated path; it is restated below, split into the three things it computes, so that
-``registration_bcpd`` runs end to end with the reference's signature and returns what the reference returns.
+``BayesianCoherentPointDrift.expectation_step`` (reference: bcpd.py:53-72) is the CPD E-step with one weight per source point and
+runs in the same two sm_90a passes (``cpd_bcpd_estep``, the ``WGT`` instantiations of the pair kernels), so the M x N matrix the
+reference materialises never exists.  ``CombinedBCPD.registration`` keeps the whole loop on the device (``cpd_bcpd_begin/step/get``):
+the float32 G^-1, the FP64 M x M precision matrix, its LU (cuSOLVER) and the posterior covariance stay resident, and per iteration
+only sigma2 and the moved source (for the reference's nearest-neighbour criterion) come back.  The host M-step below
+(``maximization_step`` / ``_maximization_step``, the reference's dense algebra restated, split into the three things it computes) is
+kept as public API, and a subclass that overrides it is driven by the host loop.
 """
 import abc
 from collections import namedtuple
@@ -159,6 +160,49 @@ class CombinedBCPD(BayesianCoherentPointDrift):
 
     def maximization_step(self, target, rigid_trans, estep_res, sigma2_p=None):
         return self._maximization_step(self._source, target, rigid_trans, estep_res, self.gmat_inv, self.lmd, self.k, sigma2_p)
+
+    def _has_device_loop(self):
+        # a subclass that brings its own E- or M-step is driven through expectation_step / maximization_step instead
+        cls = type(self)
+        return (cls.maximization_step is CombinedBCPD.maximization_step and cls._maximization_step is CombinedBCPD._maximization_step
+                and cls.expectation_step is BayesianCoherentPointDrift.expectation_step)
+
+    def registration(self, target, w=0.0, maxiter=50, tol=0.001):
+        """The loop of the reference (bcpd.py:82-101) with G^-1, the M x M precision matrix, its LU and the posterior covariance
+        resident on the GPU (cpd_bcpd_begin / cpd_bcpd_step).  Per iteration the moved source comes back for the reference's
+        stopping criterion (mean nearest-neighbour distance, cKDTree on the host), and the transformation only when a callback
+        wants it.  Returns the CombinedTransformation in the caller's point order."""
+        if not self._has_device_loop():
+            return super(CombinedBCPD, self).registration(target, w, maxiter, tol)
+        assert self._tf_type is not None, "transformation type is None."
+        cloud = _points(target)
+        state = self._initialize(cloud)
+        dim = self._source.shape[1]
+        if self._h is None or self._h.dim != dim:
+            self._h = _cabi.Handle(dim, device=self._device)
+        h = self._h
+        h.set_source(self._source)
+        h.set_target(cloud)
+        h.bcpd_begin(self.gmat_inv, self.lmd, self.k, state.sigma2, w)
+        tree = cKDTree(cloud, leafsize=10)
+        previous = None
+        for it in range(maxiter):
+            moved = h.bcpd_get(v=False, moved=True)[5]           # T(y) of the state this iteration starts from (bcpd.py:91)
+            h.bcpd_step()
+            if self._callbacks:
+                current = self._device_transformation(h)
+                for notify in self._callbacks:
+                    notify(current)
+            criterion = math_utils.compute_rmse(moved, tree)
+            log.debug("Iteration: {}, Criteria: {}".format(it, criterion))
+            if previous is not None and abs(previous - criterion) < tol:
+                break
+            previous = criterion
+        return self._device_transformation(h) if maxiter > 0 else state.transformation
+
+    def _device_transformation(self, h):
+        rot, t, scale, _, v = h.bcpd_get()[:5]
+        return self._tf_type(rot, t, scale, v)
 
     @staticmethod
     def _maximization_step(source, target, rigid_trans, estep_res, gmat_inv, lmd, k, sigma2_p=None):

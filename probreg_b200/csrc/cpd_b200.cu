@@ -5,6 +5,7 @@
 #include "kernels.cuh"
 #include "lowrank.cuh"
 #include "gram_i8.cuh"
+#include "bcpd.cuh"
 
 #include <cub/device/device_radix_sort.cuh>
 #ifdef CPD_HOST_EMU
@@ -202,11 +203,27 @@ struct cpd_ctx {
     long long nr_m = 0;
     double nr_lmd = 0.0;
     bool nr_ready = false;
-    // weighted E-step (BCPD): per-source exponent offsets and the {log2 c, dead-column shift} pair for finalize 1
+    // weighted E-step (BCPD): per-source exponent offsets (FP64 scratch, block minima, the float32 values the passes read) and
+    // {log2 c, dead-column shift, la_min} for finalize 1; d_bc_es: {scale, sigma2, w} of a stand-alone cpd_bcpd_estep
     float* d_la = nullptr;
+    double *d_la64 = nullptr, *d_la_part = nullptr, *d_bc_es = nullptr;
     size_t la_cap = 0;
     double* d_log2c = nullptr;
     bool wgt_on = false;
+    // BCPD registration loop (host_bcpd.inl): G^-1 (float32), the precision A and Sigma (FP64), all M x M in the internal order
+    BcpdState* d_bc = nullptr;
+    float* d_bc_ginv = nullptr;
+    double *d_bc_A = nullptr, *d_bc_S = nullptr, *d_bc_v = nullptr, *d_bc_r = nullptr, *d_bc_alpha = nullptr, *d_bc_sdiag = nullptr,
+           *d_bc_part = nullptr, *d_bc_sums = nullptr;
+    int64_t* d_bc_ipiv = nullptr;
+    int* d_bc_info = nullptr;             // [0] getrf's info, [1] getrs's
+    long long bc_m = 0;                   // source count the buffers were sized for
+    size_t bc_part_cap = 0;
+    double bc_sigma2 = 0.0;               // host copy of the sigma2 the next E-step uses (culling decision)
+    bool bc_ready = false;
+    bool bc_stopped = false;              // a step failed (LU, sigma2): the loop needs a new cpd_bcpd_begin
+    cudaEvent_t bc_ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+    float bc_ms[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
     // correspondence priors of ConstrainedNonRigidCPD
     double *d_wgt = nullptr, *d_p1t = nullptr, *d_pxt = nullptr;
     long long prior_m = 0;
@@ -665,8 +682,13 @@ extern "C" void cpd_destroy(cpd_ctx* h) {
     void* nrp[] = {h->d_G, h->d_W, h->d_A, h->d_B, h->d_ts2, h->d_nrpart, h->d_ipiv, h->d_info, h->d_work};
     for (void* p : nrp) if (p) cudaFree(p);
     void* lrp[] = {h->d_lr_pts, h->d_lr_Q, h->d_lr_X, h->d_lr_coef, h->d_lr_part, h->d_lr_Bc, h->d_lr_S, h->d_lr_R, h->d_lr_sys, h->d_lr_rhs,
-                   h->d_lr_c, h->d_lr_out, h->d_lr_panel, h->d_lr_Lt, h->d_gi_planes, h->d_gi_part, h->d_gi_colmax, h->d_wgt, h->d_p1t, h->d_pxt, h->d_la, h->d_log2c};
+                   h->d_lr_c, h->d_lr_out, h->d_lr_panel, h->d_lr_Lt, h->d_gi_planes, h->d_gi_part, h->d_gi_colmax, h->d_wgt, h->d_p1t, h->d_pxt, h->d_la, h->d_log2c,
+                   h->d_la64, h->d_la_part, h->d_bc_es};
     for (void* p : lrp) if (p) cudaFree(p);
+    void* bcp[] = {h->d_bc, h->d_bc_ginv, h->d_bc_A, h->d_bc_S, h->d_bc_v, h->d_bc_r, h->d_bc_alpha, h->d_bc_sdiag, h->d_bc_part, h->d_bc_sums,
+                   h->d_bc_ipiv, h->d_bc_info};
+    for (void* p : bcp) if (p) cudaFree(p);
+    for (cudaEvent_t e : h->bc_ev) if (e) cudaEventDestroy(e);
     if (h->h_work) free(h->h_work);
     if (h->sol_params && g_sol.DestroyParams) g_sol.DestroyParams(h->sol_params);
     if (h->sol && g_sol.Destroy) g_sol.Destroy(h->sol);
@@ -714,6 +736,8 @@ extern "C" int cpd_set_source(cpd_ctx* h, const double* source, int64_t m) {
         h->nr_ready = false;
     }
     TRY(ingest_cloud(h, source, m, 0, 0, nullptr, h->d_perm_src, h->d_yc));
+    h->bc_ready = false;                 // a BCPD loop starts from its own cpd_set_source + cpd_bcpd_begin
+    h->bc_stopped = false;
     h->h_state.m = m;
     h->have_source = true;
     return CPD_OK;
@@ -907,11 +931,44 @@ extern "C" int cpd_estep(cpd_ctx* h, const double* t_source, double sigma2, doub
     return cpd_last_estep(h, pt1, p1, px, n_p);
 }
 
+namespace {
+// The per-source exponents of the weighted E-step, on the device: la_m = -log2(weight_m) in FP64 (bcpd_la_kernel), their minimum,
+// the constants of finalize 1 (bcpd_la_finish_kernel) and la_m - la_min in float32 (bcpd_la_apply_kernel; perm != null: alpha and
+// sdiag are in the caller's order and are gathered into the internal one).  ssw: {scale, sigma2, w} in device memory.
+int bcpd_weights(cpd_ctx* h, const double* alpha, const double* sdiag, const int* perm, const double* ssw) {
+    const long long m = h->m;
+    const unsigned nb = blocks_for(m);
+    bcpd_la_kernel<<<nb, THREADS, 0, h->stream>>>(alpha, sdiag, m, ssw, h->dim, h->d_la64, h->d_la_part);
+    bcpd_la_finish_kernel<<<1, 32, 0, h->stream>>>(h->d_la_part, (int)nb, ssw, h->dim, h->n_global, h->d_log2c);
+    bcpd_la_apply_kernel<<<nb, THREADS, 0, h->stream>>>(h->d_la64, perm, m, h->d_log2c, h->d_la);
+    KCHECK();
+    h->launches += 3;
+    return CPD_OK;
+}
+int ensure_weight_buffers(cpd_ctx* h) {
+    const long long m = h->m;
+    if (h->la_cap < (size_t)m) {
+        TRY(dev_alloc(&h->d_la, (size_t)m));
+        TRY(dev_alloc(&h->d_la64, (size_t)m));
+        TRY(dev_alloc(&h->d_la_part, (size_t)blocks_for(m)));
+        h->la_cap = (size_t)m;
+    }
+    if (!h->d_log2c) TRY(dev_alloc(&h->d_log2c, 3));
+    if (!h->d_bc_es) TRY(dev_alloc(&h->d_bc_es, 3));
+    return CPD_OK;
+}
+}  // namespace
+
 // BayesianCoherentPointDrift.expectation_step (probreg/bcpd.py:53-72): the CPD E-step with a weight per source,
 //   pmat_nm = exp(-|x_n - t_m|^2 / 2 sigma2) (2 pi sigma2)^(-D/2) * exp(-scale^2 / (2 sigma2) * sigma_mm * D) * (1 - w) * alpha_m,
 //   den_n = w / N + sum_m pmat_nm,  P = pmat / den,  nu_d = sum_m P (n),  nu = sum_n P (m),  px = P x (m x D),  n_p = sum nu.
-// The weights enter the exponent as la_m = -log2(weight_m) (FP64 here, minus their minimum so that la >= 0 and FP32 keeps
+// The weights enter the exponent as la_m = -log2(weight_m) (FP64, minus their minimum so that la >= 0 and FP32 keeps
 // them to ~1e-7 absolute); the constant w / N moves to the same units.  x_hat = px / nu is left to the caller (bcpd.py:70-71).
+// Dead columns (bcpd.py:64-65: den == 0 -> eps, so P = 0): a term of the reference's float64 sum is exactly 0 when
+// exp(-d2 / 2 sigma2) underflows (log2 < -1075) or when its product with the factors does.  In kernel units
+// (S' = sum_m 2^-(u + la')) the first is log2 S' < -1075 -- exact for equal weights, the dominant-term approximation
+// otherwise -- and the second log2 S' - la_min - (D/2) log2(2 pi sigma2) < -1075: the smaller of the two shifts decides.
+// The exponents and constants are formed on the device by bcpd_weights, the routine the device-resident loop (host_bcpd.inl) uses.
 extern "C" int cpd_bcpd_estep(cpd_ctx* h, const double* t_source, double scale, const double* alpha, const double* sigma_diag,
                               double sigma2, double w, double* nu_d, double* nu, double* px, double* n_p) {
     if (!h || !t_source || !alpha || !sigma_diag) return fail(CPD_ERR_ARG, "null argument");
@@ -920,34 +977,25 @@ extern "C" int cpd_bcpd_estep(cpd_ctx* h, const double* t_source, double scale, 
     if (!h->have_source || !h->have_target) return fail(CPD_ERR_STATE, "source and target must both be set");
     CU(cudaSetDevice(h->device));
     const long long m = h->m;
-    std::vector<double> la((size_t)m);
-    const double kf = scale * scale / (2.0 * sigma2) * (double)h->dim * LOG2E, l1w = -log2(1.0 - w);
-    double la_min = INFINITY;
+    bool any_weight = false;
     for (long long i = 0; i < m; ++i) {
         if (!(alpha[i] >= 0.0) || !(sigma_diag[i] >= 0.0)) return fail(CPD_ERR_ARG, "alpha and diag(sigma_mat) must be non-negative");
-        la[(size_t)i] = (alpha[i] > 0.0 ? -log2(alpha[i]) : INFINITY) + l1w + kf * sigma_diag[i];
-        la_min = std::min(la_min, la[(size_t)i]);
+        any_weight = any_weight || (alpha[i] > 0.0 && sigma_diag[i] < INFINITY);
     }
-    if (!(la_min < INFINITY)) return fail(CPD_ERR_ARG, "every source has zero weight");
-    for (long long i = 0; i < m; ++i) la[(size_t)i] = std::min(la[(size_t)i] - la_min, 1.0e30);      // +inf -> a weight of exactly 0
-    if (h->la_cap < (size_t)m) { TRY(dev_alloc(&h->d_la, (size_t)m)); h->la_cap = (size_t)m; }
-    if (!h->d_log2c) TRY(dev_alloc(&h->d_log2c, 2));
-    const double half_d_log2 = 0.5 * (double)h->dim * log2(2.0 * 3.14159265358979323846 * sigma2);
-    h->h_pin[34] = (w > 0.0) ? log2(w / (double)h->n_global) + la_min + half_d_log2 : -INFINITY;   // log2 of the constant, in kernel units
-    // Dead columns (bcpd.py:64-65: den == 0 -> eps, so P = 0): a term of the reference's float64 sum is exactly 0 when
-    // exp(-d2 / 2 sigma2) underflows (log2 < -1075) or when its product with the factors does.  In kernel units
-    // (S' = sum_m 2^-(u + la')) the first is log2 S' < -1075 -- exact for equal weights, the dominant-term approximation
-    // otherwise -- and the second log2 S' - la_min - (D/2) log2(2 pi sigma2) < -1075: the smaller of the two shifts decides.
-    h->h_pin[35] = std::min(0.0, -la_min - half_d_log2);
-    CU(cudaMemcpyAsync(h->d_log2c, h->h_pin + 34, 2 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-    CU(cudaMemcpyAsync(h->d_outM, la.data(), (size_t)m * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-    gather_f32_kernel<<<blocks_for(m), THREADS, 0, h->stream>>>(h->d_outM, h->d_perm_src, m, h->d_la);
-    KCHECK();
-    CU(cudaStreamSynchronize(h->stream));          // `la` (pageable host memory) may go out of scope
+    if (!any_weight) return fail(CPD_ERR_ARG, "every source has zero weight");
+    TRY(ensure_weight_buffers(h));
+    // alpha and sigma_diag (caller's order) into d_outM [0, m) and [m, 2m), {scale, sigma2, w} into d_bc_es
+    h->h_pin[44] = scale;
+    h->h_pin[45] = sigma2;
+    h->h_pin[46] = w;
+    CU(cudaMemcpyAsync(h->d_bc_es, h->h_pin + 44, 3 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+    CU(cudaMemcpyAsync(h->d_outM, alpha, (size_t)m * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+    CU(cudaMemcpyAsync(h->d_outM + m, sigma_diag, (size_t)m * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+    TRY(bcpd_weights(h, h->d_outM, h->d_outM + m, h->d_perm_src, h->d_bc_es));
     if (h->raw_cap < (size_t)m * 3) { TRY(dev_alloc(&h->d_raw, (size_t)m * 3)); h->raw_cap = (size_t)m * 3; }
     TRY(upload_cloud(h, t_source, m, h->d_raw));
     gather3_kernel<<<blocks_for(m), THREADS, 0, h->stream>>>(h->d_raw, h->d_perm_src, m, 0.0, 0.0, 0.0, h->d_ts);
-    h->launches += 2;
+    h->launches += 1;
     TRY(ensure_stats(h));
     h->cull_active = h->extent > 0.0 && 13.3 * sqrt(sigma2) < 0.25 * h->extent;
     h->h_pin[32] = sigma2;
@@ -1035,8 +1083,9 @@ extern "C" int cpd_mstep(cpd_ctx* h, int tf_kind, int update_scale, const double
     return read_params(h, out);
 }
 
-// The remaining entry points live in four .inl files of this same translation unit:
+// The remaining entry points live in five .inl files of this same translation unit:
 #include "host_nonrigid.inl"     // cpd_nonrigid_* (dense G, low-rank factors, priors)
+#include "host_bcpd.inl"         // cpd_bcpd_begin / step / get, cpd_bcpd_step_times (the BCPD loop on the device)
 #include "host_stateless.inl"    // cpd_rbf_kernel, cpd_imq_kernel, cpd_gauss_transform, cpd_squared_kernel_sum
 #include "host_multi.inl"        // cpd_comm_*, cpd_p2p_*
 #include "host_measure.inl"      // cpd_timer_*, cpd_event_*, cpd_stage_times, cpd_flush_l2, cpd_microbench
