@@ -119,6 +119,19 @@ int cpd_bcpd_step(cpd_ctx* h, double* sigma2_out);
 /* The current state, caller's order; any pointer may be NULL.  sim: lin = rot, t, scale, sigma2 (n_p: of the last E-step).
  * v_out, moved_out (s R (y + v) + t): m x D;  alpha_out, sigma_diag_out: m.                                                    */
 int cpd_bcpd_get(cpd_ctx* h, cpd_params* sim, double* v_out, double* moved_out, double* alpha_out, double* sigma_diag_out);
+/* The same loop with the kernel matrix replaced by a rank-K factorisation G ~= Q Bc Q^T of the inverse multiquadric
+ * G_ij = (|y_i - y_j|^2 + c)^(-1/2) (CombinedBCPD uses c = 1): no G^-1, nothing of size M x M on the device or the host, and a
+ * K x K M-step (csrc/bcpd.cuh).  Sound where G is numerically of low rank -- source clouds of extent up to a few sqrt(c); the dense
+ * loop above stays for the others.  The factors come from the low-rank set-up of cpd_nonrigid_lowrank_begin (randomised range
+ * finder, `power_iters` subspace iterations, seeded) with the IMQ kernel; set-up times go to cpd_lowrank_setup_times.
+ * Same preconditions and starting state as cpd_bcpd_begin; c > 0, rank 1..1024 (clamped to m), power_iters 0..8.
+ * cpd_bcpd_step / cpd_bcpd_get then run and read the low-rank loop, with the same failure rules (a singular K x K factor, a failed
+ * solve or a sigma2 that is not a positive finite number stop it until the next begin).  The handle's low-rank factors are
+ * shared with non-rigid CPD: this call ends a non-rigid loop on the handle, a later cpd_nonrigid_*begin ends this loop (its next
+ * step fails and says why), and cpd_bcpd_begin returns the handle to the dense loop.
+ * cpd_bcpd_lowrank_get: the rank in use, Q (m x rank, row-major, caller's order) and Bc = L L^T (rank x rank); any may be NULL.  */
+int cpd_bcpd_lowrank_begin(cpd_ctx* h, double c, double lmd, double k, double sigma2, double w, int rank, int power_iters, uint64_t seed);
+int cpd_bcpd_lowrank_get(cpd_ctx* h, int* rank_out, double* q_out, double* bcore_out);
 
 /* Copies of the last E-step's reductions (device -> host), valid after cpd_em_step/run. */
 int cpd_last_estep(cpd_ctx* h, double* pt1, double* p1, double* px, double* n_p);
@@ -146,8 +159,9 @@ int cpd_nonrigid_mstep(cpd_ctx* h, const double* pt1, const double* p1, const do
  * the default form: positive semi-definite, exactly the core the iteration uses); any may be NULL. */
 int cpd_nonrigid_lowrank_begin(cpd_ctx* h, double beta, double lmd, double sigma2, double w, int rank, int power_iters, uint64_t seed);
 int cpd_nonrigid_lowrank_get(cpd_ctx* h, int* rank_out, double* q_out, double* bcore_out);
-/* Test / diagnostic entry (like cpd_plan_work): out = G x for the G of the last cpd_nonrigid_lowrank_begin on this handle (its beta
- * and source points; the source must not have changed since).  x and out are m x cols (1 <= cols <= 1024), row-major, in the
+/* Test / diagnostic entry (like cpd_plan_work): out = G x for the G of the last low-rank set-up on this handle: the Gaussian of
+ * cpd_nonrigid_lowrank_begin's beta or the inverse multiquadric of cpd_bcpd_lowrank_begin's c, on its source points (the source
+ * must not have changed since).  x and out are m x cols (1 <= cols <= 1024), row-major, in the
  * caller's point order.  kernel 0: the exact integer-digit product on the tensor cores (csrc/gram_i8.cuh), 1: the CUDA-core kernel
  * (csrc/lowrank.cuh); the call goes straight to it, without the first-use self-check.  world = 1, rank = 0: every row; otherwise
  * only the rows that rank `rank` of a `world`-rank handle forms are filled and the others are zero (there is no exchange).  The
@@ -220,9 +234,11 @@ int cpd_event_elapsed(cpd_ctx* h, int idx_start, int idx_stop, float* ms);
 int cpd_set_profiling(cpd_ctx* h, int on);
 int cpd_stage_times(cpd_ctx* h, float ms[6]);
 /* the last cpd_bcpd_step run with profiling on, ms: [0] E-step [1] building the precision matrix [2] getrf [3] getrs against the
- * identity [4] the rest of the M-step                                                                                          */
+ * identity [4] the rest of the M-step.  In low-rank mode: [0] E-step [1] St and Rt (and the K x K system) [2] getrf (K) [3] getrs (K)
+ * [4] the rest (v, diag Sigma, mixing weights, similarity, sigma2)                                                              */
 int cpd_bcpd_step_times(cpd_ctx* h, float ms[5]);
-/* the last cpd_nonrigid_lowrank_begin run with profiling on: ms of [0] the G X products [1] the orthonormalisations [2] Bc       */
+/* the last low-rank set-up (cpd_nonrigid_lowrank_begin or cpd_bcpd_lowrank_begin) run with profiling on: ms of [0] the G X
+ * products [1] the orthonormalisations [2] Bc and its factor                                                                     */
 int cpd_lowrank_setup_times(cpd_ctx* h, float ms[3]);
 /* launches issued by this handle since creation (kernels only).                         */
 int64_t cpd_launch_count(cpd_ctx* h);

@@ -47,6 +47,9 @@ _PROTOS = {
     "cpd_bcpd_step": (ctypes.c_int, [ctypes.c_void_p, _c_dp]),
     "cpd_bcpd_get": (ctypes.c_int, [ctypes.c_void_p, ctypes.POINTER(CpdParams), _c_dp, _c_dp, _c_dp, _c_dp]),
     "cpd_bcpd_step_times": (ctypes.c_int, [ctypes.c_void_p, _c_fp]),
+    "cpd_bcpd_lowrank_begin": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_double, ctypes.c_double, ctypes.c_double, ctypes.c_double,
+                                              ctypes.c_double, ctypes.c_int, ctypes.c_int, ctypes.c_uint64]),
+    "cpd_bcpd_lowrank_get": (ctypes.c_int, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_int), _c_dp, _c_dp]),
     "cpd_nonrigid_begin": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_double, ctypes.c_double, ctypes.c_double, ctypes.c_double]),
     "cpd_nonrigid_step": (ctypes.c_int, [ctypes.c_void_p, _c_dp]),
     "cpd_nonrigid_get": (ctypes.c_int, [ctypes.c_void_p, _c_dp, _c_dp]),
@@ -247,6 +250,29 @@ class Handle(object):
             raise ValueError("gmat_inv must be C-contiguous (row-major)")
         check(self._lib.cpd_bcpd_begin(self._h, gmat_inv.ctypes.data_as(_c_fp), float(lmd), float(k), float(sigma2), float(w)))
 
+    def bcpd_lowrank_begin(self, c, lmd, k, sigma2, w, rank, power_iters=2, seed=0):
+        """Start CombinedBCPD's loop with the IMQ kernel matrix (parameter c) replaced by a rank-`rank` factorisation built on the
+        device (set_source / set_target first); bcpd_step / bcpd_get then run the low-rank loop."""
+        for name, val in (("rank", rank), ("power_iters", power_iters), ("seed", seed)):
+            if isinstance(val, bool) or not isinstance(val, (int, np.integer)):
+                raise ValueError("%s must be an integer, got %r" % (name, val))
+        if not 1 <= rank <= 1024:
+            raise ValueError("rank must be in 1..1024, got %d" % rank)
+        if not 0 <= power_iters <= 8:
+            raise ValueError("power_iters must be in 0..8, got %d" % power_iters)
+        if not (np.isfinite(c) and c > 0):
+            raise ValueError("c must be a positive finite number, got %r" % (c,))
+        check(self._lib.cpd_bcpd_lowrank_begin(self._h, float(c), float(lmd), float(k), float(sigma2), float(w), int(rank), int(power_iters),
+                                               int(seed)))
+
+    def bcpd_lowrank_factors(self):
+        """(Q (m x rank), Bc (rank x rank)) of the low-rank BCPD loop: G ~= Q Bc Q^T, Q in the caller's point order."""
+        k = ctypes.c_int()
+        check(self._lib.cpd_bcpd_lowrank_get(self._h, ctypes.byref(k), None, None))
+        q, b = np.empty((self.m, k.value)), np.empty((k.value, k.value))
+        check(self._lib.cpd_bcpd_lowrank_get(self._h, None, dptr(q), dptr(b)))
+        return q, b
+
     def bcpd_step(self):
         """One iteration; returns the new sigma2."""
         out = ctypes.c_double()
@@ -306,7 +332,8 @@ class Handle(object):
     GRAM_TENSOR_CORES, GRAM_CUDA_CORES = 0, 1
 
     def lowrank_gram_product(self, x, kernel, world=1, rank=0):
-        """G x (m x cols) for the G of the last nonrigid_lowrank_begin, by one kernel (GRAM_TENSOR_CORES or GRAM_CUDA_CORES);
+        """G x (m x cols) for the G of the last low-rank set-up (nonrigid_lowrank_begin: Gaussian, bcpd_lowrank_begin: inverse
+        multiquadric), by one kernel (GRAM_TENSOR_CORES or GRAM_CUDA_CORES);
         with world > 1 only the rows of `rank`'s share are filled.  A test / diagnostic entry: the factors stay as they were."""
         xa = np.ascontiguousarray(x, dtype=np.float64)
         if xa.ndim != 2 or xa.shape[0] != self.m:

@@ -4,7 +4,9 @@
 runs in the same two sm_90a passes (``cpd_bcpd_estep``, the ``WGT`` instantiations of the pair kernels), so the M x N matrix the
 reference materialises never exists.  ``CombinedBCPD.registration`` keeps the whole loop on the device (``cpd_bcpd_begin/step/get``):
 the float32 G^-1, the FP64 M x M precision matrix, its LU (cuSOLVER) and the posterior covariance stay resident, and per iteration
-only sigma2 and the moved source (for the reference's nearest-neighbour criterion) come back.  The host M-step below
+only sigma2 and the moved source (for the reference's nearest-neighbour criterion) come back.  ``CombinedBCPD(low_rank=K)`` replaces
+the kernel matrix by a rank-K factorisation built on the device (``cpd_bcpd_lowrank_begin``): no G^-1 and nothing of size M x M, a
+K x K M-step, for clouds whose kernel matrix is numerically of low rank (extent up to a few sqrt(c)).  The host M-step below
 (``maximization_step`` / ``_maximization_step``, the reference's dense algebra restated, split into the three things it computes) is
 kept as public API, and a subclass that overrides it is driven by the host loop.
 """
@@ -143,22 +145,41 @@ class CombinedBCPD(BayesianCoherentPointDrift):
 
     lmd -- weight of the motion-coherence prior;  k -- Dirichlet concentration of the mixing weights;  gamma -- factor on the
     initial sigma2;  device -- CUDA ordinal (extension).
+    low_rank -- None (the dense loop) or the rank K of a factorisation G ~= Q Bc Q^T of the inverse-multiquadric kernel matrix
+    (c = 1), built on the device by a randomised range finder with ``low_rank_iters`` subspace iterations from ``low_rank_seed``; the
+    loop then runs with K x K algebra and nothing of size M x M.  Suited to clouds of extent up to about 3 (in the kernel's units,
+    sqrt(c) = 1), where G is numerically of low rank; the dense loop remains for the others.  The host M-step stays dense only.
     """
 
-    def __init__(self, source=None, lmd=2.0, k=1.0e20, gamma=1.0, device=0):
+    def __init__(self, source=None, lmd=2.0, k=1.0e20, gamma=1.0, device=0, low_rank=None, low_rank_iters=2, low_rank_seed=0):
         super(CombinedBCPD, self).__init__(source, device)
         self._tf_type = tf.CombinedTransformation
         self.lmd, self.k, self.gamma = lmd, k, gamma
+        if low_rank is not None and (isinstance(low_rank, bool) or not isinstance(low_rank, (int, np.integer)) or low_rank < 1):
+            raise ValueError("low_rank must be None or a positive integer, got %r" % (low_rank,))
+        self.low_rank, self.low_rank_iters, self.low_rank_seed = low_rank, low_rank_iters, low_rank_seed
+        self._check_low_rank()
+
+    def _check_low_rank(self):
+        if self.low_rank is not None and not self._has_device_loop():
+            raise ValueError("low_rank runs on the device loop only: %s overrides the E- or M-step, which stay dense"
+                             % type(self).__name__)
 
     def _initialize(self, target):
         count, dim = self._source.shape
-        self.gmat = math_utils.inverse_multiquadric_kernel(self._source, self._source, device=self._device)
-        self.gmat_inv = np.linalg.inv(self.gmat)
         start_var = self.gamma * math_utils.squared_kernel_sum(self._source, target, device=self._device)
         identity_map = self._tf_type(np.identity(dim), np.zeros(dim))
+        if self.low_rank is not None:
+            # nothing of size M x M: the factors are built on the device, and only the diagonal of sigma_mat is kept
+            self.gmat = self.gmat_inv = None
+            return MstepResult(identity_map, None, np.ones(count), 1.0 / count, start_var)
+        self.gmat = math_utils.inverse_multiquadric_kernel(self._source, self._source, device=self._device)
+        self.gmat_inv = np.linalg.inv(self.gmat)
         return MstepResult(identity_map, None, np.identity(count), 1.0 / count, start_var)
 
     def maximization_step(self, target, rigid_trans, estep_res, sigma2_p=None):
+        if self.low_rank is not None:
+            raise ValueError("the host M-step is dense only: it is not available with low_rank")
         return self._maximization_step(self._source, target, rigid_trans, estep_res, self.gmat_inv, self.lmd, self.k, sigma2_p)
 
     def _has_device_loop(self):
@@ -169,9 +190,10 @@ class CombinedBCPD(BayesianCoherentPointDrift):
 
     def registration(self, target, w=0.0, maxiter=50, tol=0.001):
         """The loop of the reference (bcpd.py:82-101) with G^-1, the M x M precision matrix, its LU and the posterior covariance
-        resident on the GPU (cpd_bcpd_begin / cpd_bcpd_step).  Per iteration the moved source comes back for the reference's
+        resident on the GPU (cpd_bcpd_begin / cpd_bcpd_step), or with low_rank the K x K loop (cpd_bcpd_lowrank_begin).  Per iteration the moved source comes back for the reference's
         stopping criterion (mean nearest-neighbour distance, cKDTree on the host), and the transformation only when a callback
         wants it.  Returns the CombinedTransformation in the caller's point order."""
+        self._check_low_rank()
         if not self._has_device_loop():
             return super(CombinedBCPD, self).registration(target, w, maxiter, tol)
         assert self._tf_type is not None, "transformation type is None."
@@ -183,7 +205,10 @@ class CombinedBCPD(BayesianCoherentPointDrift):
         h = self._h
         h.set_source(self._source)
         h.set_target(cloud)
-        h.bcpd_begin(self.gmat_inv, self.lmd, self.k, state.sigma2, w)
+        if self.low_rank is not None:
+            h.bcpd_lowrank_begin(1.0, self.lmd, self.k, state.sigma2, w, self.low_rank, self.low_rank_iters, self.low_rank_seed)
+        else:
+            h.bcpd_begin(self.gmat_inv, self.lmd, self.k, state.sigma2, w)
         tree = cKDTree(cloud, leafsize=10)
         previous = None
         for it in range(maxiter):
@@ -226,7 +251,7 @@ def registration_bcpd(source, target, w=0.0, maxiter=50, tol=0.001, callbacks=()
 
     source, target: (M, D) / (N, D) arrays (or open3d point clouds);  w: outlier probability;  maxiter / tol: EM budget and the
     tolerance on the nearest-neighbour criterion;  callbacks: callables taking the current transformation;  kwargs go to
-    ``CombinedBCPD`` (lmd, k, gamma, device).  Returns the estimated ``CombinedTransformation``.
+    ``CombinedBCPD`` (lmd, k, gamma, device, low_rank, low_rank_iters, low_rank_seed).  Returns the estimated ``CombinedTransformation``.
     """
     solver = CombinedBCPD(_points(source), **kwargs)
     solver.set_callbacks(list(callbacks))

@@ -13,8 +13,11 @@
 //               -- evaluated in the targets' centred frame (x - cx, yhat - cx): the same value, since sum nu_d = sum nu and
 //               sum_n nu_d x_n = sum_m px_m, without the centroid offset in the cancellation.
 // All vectors are in the library's internal (Z-order) source order; the M x M matrices are row-major in that order.
+// The low-rank loop (cpd_bcpd_lowrank_begin) replaces the precision, covariance and displacement steps by the K x K algebra at the
+// end of this file.
 #pragma once
 #include "kernels.cuh"
+#include "lowrank.cuh"
 
 namespace cpd {
 
@@ -109,23 +112,27 @@ bcpd_system_kernel(const float* __restrict__ ginv, const double* __restrict__ nu
     }
 }
 
-// r_m = R^T (px_m - nu_m t) / s - nu_m y_m  (m x 3), px = pxc + nu cx, y = yc + cy
+// r_i = R^T (px_i - nu_i t) / s - nu_i y_i, px = pxc + nu cx, y = yc + cy; element a is stored at r[a * stride_a + i * stride_i]
+__device__ __forceinline__ void bcpd_rhs_point(const BcpdState* __restrict__ bc, const DevState* __restrict__ st, const double* __restrict__ nu,
+                                               const double* __restrict__ pxc, const double* __restrict__ yc, long long i, double* __restrict__ r,
+                                               long long stride_a, long long stride_i) {
+    const double n = nu[i];
+    double q[3];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) q[a] = pxc[3 * i + a] + n * (st->cx[a] - bc->t[a]);
+    const double inv_s = 1.0 / bc->scale;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+        const double rt = bc->rot[a] * q[0] + bc->rot[3 + a] * q[1] + bc->rot[6 + a] * q[2];      // (R^T q)_a
+        r[a * stride_a + i * stride_i] = rt * inv_s - n * (yc[3 * i + a] + st->cy[a]);
+    }
+}
+// r (m x 3, point-major) for the dense M-step
 __global__ void __launch_bounds__(THREADS)
 bcpd_rhs_kernel(const BcpdState* __restrict__ bc, const DevState* __restrict__ st, const double* __restrict__ nu,
                 const double* __restrict__ pxc, const double* __restrict__ yc, long long m, double* __restrict__ r) {
     const long long i = (long long)blockIdx.x * THREADS + threadIdx.x;
-    if (i < m) {
-        const double n = nu[i];
-        double q[3];
-#pragma unroll
-        for (int a = 0; a < 3; ++a) q[a] = pxc[3 * i + a] + n * (st->cx[a] - bc->t[a]);
-        const double inv_s = 1.0 / bc->scale;
-#pragma unroll
-        for (int a = 0; a < 3; ++a) {
-            const double rt = bc->rot[a] * q[0] + bc->rot[3 + a] * q[1] + bc->rot[6 + a] * q[2];      // (R^T q)_a
-            r[3 * i + a] = rt * inv_s - n * (yc[3 * i + a] + st->cy[a]);
-        }
-    }
+    if (i < m) bcpd_rhs_point(bc, st, nu, pxc, yc, i, r, 1, 3);
 }
 
 // v_i = ratio sum_j Sigma_ij r_j (one warp per row, FP64) and sdiag_i = Sigma_ii
@@ -288,6 +295,66 @@ __global__ void __launch_bounds__(THREADS)
 bcpd_fill_kernel(double* __restrict__ x, long long count, double value) {
     const long long k = (long long)blockIdx.x * THREADS + threadIdx.x;
     if (k < count) x[k] = value;
+}
+
+// ---- the low-rank M-step (cpd_bcpd_lowrank_begin) ---------------------------------------------------------------------------------
+// With G ~= Qt Qt^T (Qt = Q L of the set-up, lowrank.cuh: [K][ld], K columns) the displacement is v = Qt w with the prior
+// w ~ N(0, I / lmd).  The posterior of w given the E-step is Gaussian with precision ratio (c I + St):
+//     c = lmd / ratio,   St = Qt^T diag(nu) Qt,   C = (c I + St)^-1      (symmetric positive definite, eigenvalues of C^-1 >= c)
+//     v = Qt C Rt,   Rt = Qt^T r      (r of bcpd_rhs_point: nu (T^-1(x_hat) - y) without dividing by nu)
+//     diag Sigma_v = diag(Qt C Qt^T) / ratio = sum_k Qt[k][i] (C Qt^T)[k][i] / ratio      (FP64, >= 0, no M x M buffer)
+// At K = M with Qt of full rank this is (lmd G^-1 + ratio diag(nu))^-1: the dense loop's Sigma.  No G^-1, no Bc^-1, no division by
+// nu: a source no target explains keeps a finite v, and a column the pivoted Cholesky dropped (zero in Qt) gives St a zero row and
+// column, where C = 1 / c.  Mixing weights, similarity and sigma2 follow with the dense loop's kernels.
+
+// r in the [3][m] layout lr_inner_narrow_kernel reads
+__global__ void __launch_bounds__(THREADS)
+bcpd_lr_rhs_kernel(const BcpdState* __restrict__ bc, const DevState* __restrict__ st, const double* __restrict__ nu,
+                   const double* __restrict__ pxc, const double* __restrict__ yc, long long m, double* __restrict__ r) {
+    const long long i = (long long)blockIdx.x * THREADS + threadIdx.x;
+    if (i < m) bcpd_rhs_point(bc, st, nu, pxc, yc, i, r, m, 1);
+}
+// Msys = c I + St (row-major K x K), c = lmd / ratio from the loop state, and E = I, the right-hand side the solve overwrites with C
+__global__ void __launch_bounds__(THREADS)
+bcpd_lr_system_kernel(const double* __restrict__ St, const BcpdState* __restrict__ bc, int K, double* __restrict__ Msys, double* __restrict__ E) {
+    const long long e = (long long)blockIdx.x * THREADS + threadIdx.x;
+    if (e < (long long)K * K) {
+        const double q = bc->scale / bc->sigma2, c = bc->lmd / (q * q);
+        const bool diag = e / K == e % K;
+        Msys[e] = St[e] + (diag ? c : 0.0);
+        E[e] = diag ? 1.0 : 0.0;
+    }
+}
+// w[k][d] = sum_b C[k][b] Rt[b][d]   (K x 3; Rt as lr_merge_kernel leaves it, [K][3])
+__global__ void __launch_bounds__(THREADS)
+bcpd_lr_coef_kernel(const double* __restrict__ C, const double* __restrict__ Rt, int K, double* __restrict__ w) {
+    const int e = blockIdx.x * THREADS + threadIdx.x;
+    if (e < 3 * K) {
+        const int k = e / 3, d = e % 3;
+        double s = 0.0;
+        for (int b = 0; b < K; ++b) s = fma(C[(size_t)k * K + b], Rt[(size_t)b * 3 + d], s);
+        w[e] = s;
+    }
+}
+// v_i = sum_k Qt[k][i] w[k]  (m x 3, point-major) and sdiag_i = sum_k Qt[k][i] CQ[k][i] / ratio, CQ = C Qt^T (lr_rotate_kernel)
+__global__ void __launch_bounds__(THREADS)
+bcpd_lr_disp_kernel(const double* __restrict__ Qt, const double* __restrict__ CQ, long long ld, int K, const double* __restrict__ w,
+                    const BcpdState* __restrict__ bc, long long m, double* __restrict__ v, double* __restrict__ sdiag) {
+    __shared__ double sw[3 * LR_MAX_RANK];
+    for (int e = threadIdx.x; e < 3 * K; e += THREADS) sw[e] = w[e];
+    __syncthreads();
+    const long long i = (long long)blockIdx.x * THREADS + threadIdx.x;
+    if (i < m) {
+        double a0 = 0.0, a1 = 0.0, a2 = 0.0, sd = 0.0;
+        for (int k = 0; k < K; ++k) {
+            const double q = Qt[(long long)k * ld + i];
+            a0 = fma(q, sw[3 * k], a0); a1 = fma(q, sw[3 * k + 1], a1); a2 = fma(q, sw[3 * k + 2], a2);
+            sd = fma(q, CQ[(long long)k * ld + i], sd);
+        }
+        const double r = bc->scale / bc->sigma2;
+        v[3 * i] = a0; v[3 * i + 1] = a1; v[3 * i + 2] = a2;
+        sdiag[i] = sd / (r * r);
+    }
 }
 
 }  // namespace cpd

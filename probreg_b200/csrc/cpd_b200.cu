@@ -203,6 +203,7 @@ struct cpd_ctx {
     long long nr_m = 0;
     double nr_lmd = 0.0;
     bool nr_ready = false;
+    bool nr_lost_to_bcpd = false;         // the non-rigid loop ended because cpd_bcpd_lowrank_begin took the low-rank factors
     // weighted E-step (BCPD): per-source exponent offsets (FP64 scratch, block minima, the float32 values the passes read) and
     // {log2 c, dead-column shift, la_min} for finalize 1; d_bc_es: {scale, sigma2, w} of a stand-alone cpd_bcpd_estep
     float* d_la = nullptr;
@@ -224,6 +225,14 @@ struct cpd_ctx {
     bool bc_stopped = false;              // a step failed (LU, sigma2): the loop needs a new cpd_bcpd_begin
     cudaEvent_t bc_ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     float bc_ms[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
+    long long bc_vec_m = 0, bc_dense_m = 0;   // source counts of the per-source vectors and of the three M x M buffers
+    // low-rank mode (cpd_bcpd_lowrank_begin): the factor is the handle's low-rank Qt (d_lr_X); the K x K system and C = its
+    // inverse, C Qt^T ([K][ld]), r in [3][m], w = C Rt (K x 3) and the pivots of the K x K LU
+    bool bc_lowrank = false;
+    double *d_bc_sys = nullptr, *d_bc_C = nullptr, *d_bc_CQ = nullptr, *d_bc_rt = nullptr, *d_bc_w = nullptr;
+    int64_t* d_bc_lr_ipiv = nullptr;
+    long long bc_lr_m = 0;
+    int bc_lr_k = 0;
     // correspondence priors of ConstrainedNonRigidCPD
     double *d_wgt = nullptr, *d_p1t = nullptr, *d_pxt = nullptr;
     long long prior_m = 0;
@@ -231,6 +240,8 @@ struct cpd_ctx {
     bool prior_on = false;
     // non-rigid CPD, rank-K G ~= Q Bc Q^T (lowrank.cuh)
     int lr_rank = 0;                      // > 0: cpd_nonrigid_step takes the low-rank M-step
+    int lr_owner = 0;                     // whose set-up the factors are: LR_OWNER_NONE / _NONRIGID (Gaussian G) / _BCPD (IMQ G)
+    double lr_gscale = 1.0;               // the factor of the products beyond the tile values: c^(-1/2) for the IMQ, 1 for the Gaussian
     bool lr_w_stale = false;              // W of the low-rank path is formed on demand
     float lr_setup_ms[3] = {0.f, 0.f, 0.f};   // products / orthonormalisations / core of the last profiled set-up
     long long lr_m = 0;
@@ -686,7 +697,7 @@ extern "C" void cpd_destroy(cpd_ctx* h) {
                    h->d_la64, h->d_la_part, h->d_bc_es};
     for (void* p : lrp) if (p) cudaFree(p);
     void* bcp[] = {h->d_bc, h->d_bc_ginv, h->d_bc_A, h->d_bc_S, h->d_bc_v, h->d_bc_r, h->d_bc_alpha, h->d_bc_sdiag, h->d_bc_part, h->d_bc_sums,
-                   h->d_bc_ipiv, h->d_bc_info};
+                   h->d_bc_ipiv, h->d_bc_info, h->d_bc_sys, h->d_bc_C, h->d_bc_CQ, h->d_bc_rt, h->d_bc_w, h->d_bc_lr_ipiv};
     for (void* p : bcp) if (p) cudaFree(p);
     for (cudaEvent_t e : h->bc_ev) if (e) cudaEventDestroy(e);
     if (h->h_work) free(h->h_work);

@@ -3,7 +3,8 @@
 // signed 8-bit, 32-bit integer accumulators in registers).  Integer MMAs do not round, so the only errors are the two
 // quantisations (2^-24 absolute on G, 2^-23 of the column maximum on X), at the level of the float32 G the reference itself uses
 // (cc/math_utils.cc:17-19).  Role: the products of the low-rank range finder (probreg/cpd.py:296-297 with
-// G = rbf_kernel(Y, Y, beta) of transformation.py:91-102); G is never stored -- it is generated tile by tile on the CUDA cores.
+// G = rbf_kernel(Y, Y, beta) of transformation.py:91-102) and, as the LR_IMQ instantiation, of low-rank BCPD (the inverse multiquadric,
+// lowrank.cuh); G is never stored -- it is generated tile by tile on the CUDA cores.
 //
 // Fixed point ("Ozaki splitting" with integer digits):
 //     g_ij = round(2^23 G_ij) in [0, 2^23]         = a0 2^16 + a1 2^8 + a2,     a_s in [0, 255]        (unsigned digits, a0 <= 128)
@@ -161,9 +162,11 @@ gi_compare_kernel(const double* __restrict__ a, const double* __restrict__ b, lo
 // one column pass: images = the stage images of gi_split_kernel (jpad / 32 of them); pts: float4 {a, 0} per point in the scaled frame
 // of lr_pack_kernel, padded to jpad with far-away records (G == 0); rows [i_begin, i_end) of G;
 // part[q][c][ii] (FP64) = colmax[c] 2^-45 sum_{j in chunk q} g_ij x_cj  for c < GI_N, ii < ldp (a multiple of GI_ROWS)
+// KIND: the tile values of lr_kernel_value (lowrank.cuh); for LR_IMQ the epilogue scale also carries gscale = c^(-1/2).
+template <int KIND>
 __global__ void __launch_bounds__(GI_THREADS, 1)
 gi_gram_kernel(const unsigned char* __restrict__ images, const float4* __restrict__ pts, long long jpad, int chunk, long long i_begin,
-               long long i_end, const double* __restrict__ colmax, double* __restrict__ part, long long ldp) {
+               long long i_end, const double* __restrict__ colmax, double* __restrict__ part, long long ldp, double gscale) {
     // 256-byte alignment anchors the 32-byte swizzle pattern of every B plane the way the MMA unit reads it
     extern __shared__ __align__(256) unsigned char gi_smem_raw[];
     unsigned char* planes = gi_smem_raw;                                      // [GI_STAGES][3][GI_PLANE]
@@ -240,7 +243,7 @@ gi_gram_kernel(const unsigned char* __restrict__ images, const float4* __restric
                 for (int h = 0; h < 2; ++h) {
                     const float dx = __fsub_rn(ax[h], b.x), dy = __fsub_rn(ay[h], b.y), dz = __fsub_rn(az[h], b.z);
                     const float uu = __fmaf_rn(dz, dz, __fmaf_rn(dy, dy, __fmul_rn(dx, dx)));
-                    const float e = ex2(-uu);                   // the same float32 G as the other kernels; G = 1 gives the digits (128, 0, 0)
+                    const float e = lr_kernel_value<KIND>(uu);  // the same float32 G as the other kernels; G = 1 gives the digits (128, 0, 0)
                     gq[h][s] = __float_as_uint(__fmaf_rn(e, 8388608.0f, 8388608.0f));
                 }
             }
@@ -278,7 +281,8 @@ gi_gram_kernel(const unsigned char* __restrict__ images, const float4* __restric
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int c = 8 * i + 2 * (lane & 3) + h;
-                const double sc = colmax[c] * (1.0 / 536870912.0);                                 // 2^16 2^-45
+                double sc = colmax[c] * (1.0 / 536870912.0);                                       // 2^16 2^-45
+                if constexpr (KIND == LR_IMQ) sc *= gscale;
 #pragma unroll
                 for (int rr = 0; rr < 2; ++rr) {
                     const int k = 4 * i + 2 * rr + h;
