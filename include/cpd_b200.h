@@ -133,6 +133,34 @@ int cpd_bcpd_get(cpd_ctx* h, cpd_params* sim, double* v_out, double* moved_out, 
 int cpd_bcpd_lowrank_begin(cpd_ctx* h, double c, double lmd, double k, double sigma2, double w, int rank, int power_iters, uint64_t seed);
 int cpd_bcpd_lowrank_get(cpd_ctx* h, int* rank_out, double* q_out, double* bcore_out);
 
+/* GMMTree (probreg/gmmtree.py, probreg/cc/gmmtree.cc; csrc/gmmtree.cuh), 3-D only, one GPU (a handle with a communicator attached
+ * is refused with CPD_ERR_STATE).  A tree of tree_level = L (1..5) levels has n_total = 8 (8^L - 1) / 7 nodes (pi, mu, Sigma);
+ * level l holds the 8^(l+1) nodes from 8 (8^l - 1) / 7, and the children of node j start at 8 (j + 1).
+ * cpd_gmmtree_build: buildGmmTree on the handle's source, in FP64 (pdfs, log-likelihood, moments), every reduction in a fixed
+ * order (bit-identical runs on one device).  Where it departs from the reference: the 8^L leaves are seeded from leaf_seeds
+ * (8^L point indices into the source, caller's order) instead of Eigen's random draw, which reads out of bounds for L >= 2; and
+ * each level stops after maxiter (>= 1) EM iterations if |q - q_prev| < lambda_s has not stopped it before.  iters_per_level (L
+ * ints, may be NULL): the iterations each level ran.  lambda_d: the m0 below which a node dies (the reference passes 1e-4).
+ * The tree does not depend on the source once built: cpd_set_source keeps it.
+ * cpd_gmmtree_nodes: the current tree, pi (n_total), mu (n_total x 3), cov (n_total x 3 x 3), in the caller's coordinates; any
+ * may be NULL.  cpd_gmmtree_load installs a caller's tree of the same layout instead (all finite) -- to test the E-step alone.
+ * cpd_gmmtree_assign: per source point (caller's order, m int32) the node it was assigned to in the last E-step of the build's
+ * last level (the leaf level); refused after a load or once the source count has changed.
+ * cpd_gmmtree_estep: gmmTreeRegEstep on the handle's target moved by z = rot x + t (rot row-major 3 x 3): each point descends
+ * from the root to the argmax child until a node of complexity (smallest eigenvalue / trace of Sigma) <= lambda_c, and adds
+ * (gamma, gamma z, gamma z z^T) to that node only.  moments: n_total x 13 (m0, m1[3], m2[3][3] row-major).
+ * cpd_gmmtree_times: with profiling on (cpd_set_profiling), ms of each level of the last build (level_ms[l], l < L; 0 beyond)
+ * and of the last cpd_gmmtree_estep; either pointer may be NULL.
+ * Refused with CPD_ERR_ARG: a 2-D handle, tree_level outside 1..5, a seed outside 0..m-1, a non-finite parameter, source or
+ * target; with CPD_ERR_STATE: no source (build), no tree or no target (E-step).                                                */
+int cpd_gmmtree_build(cpd_ctx* h, int tree_level, double lambda_s, double lambda_d, const int64_t* leaf_seeds, int maxiter,
+                      int* iters_per_level);
+int cpd_gmmtree_nodes(cpd_ctx* h, double* pi, double* mu, double* cov);
+int cpd_gmmtree_load(cpd_ctx* h, int tree_level, const double* pi, const double* mu, const double* cov);
+int cpd_gmmtree_assign(cpd_ctx* h, int32_t* node);
+int cpd_gmmtree_estep(cpd_ctx* h, const double rot[9], const double t[3], double lambda_c, double* moments);
+int cpd_gmmtree_times(cpd_ctx* h, float level_ms[5], float* estep_ms);
+
 /* Copies of the last E-step's reductions (device -> host), valid after cpd_em_step/run. */
 int cpd_last_estep(cpd_ctx* h, double* pt1, double* p1, double* px, double* n_p);
 

@@ -50,6 +50,13 @@ _PROTOS = {
     "cpd_bcpd_lowrank_begin": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_double, ctypes.c_double, ctypes.c_double, ctypes.c_double,
                                               ctypes.c_double, ctypes.c_int, ctypes.c_int, ctypes.c_uint64]),
     "cpd_bcpd_lowrank_get": (ctypes.c_int, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_int), _c_dp, _c_dp]),
+    "cpd_gmmtree_build": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_double, ctypes.c_double, ctypes.POINTER(ctypes.c_int64),
+                                         ctypes.c_int, ctypes.POINTER(ctypes.c_int)]),
+    "cpd_gmmtree_nodes": (ctypes.c_int, [ctypes.c_void_p, _c_dp, _c_dp, _c_dp]),
+    "cpd_gmmtree_load": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, _c_dp, _c_dp, _c_dp]),
+    "cpd_gmmtree_assign": (ctypes.c_int, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_int32)]),
+    "cpd_gmmtree_estep": (ctypes.c_int, [ctypes.c_void_p, _c_dp, _c_dp, ctypes.c_double, _c_dp]),
+    "cpd_gmmtree_times": (ctypes.c_int, [ctypes.c_void_p, _c_fp, _c_fp]),
     "cpd_nonrigid_begin": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_double, ctypes.c_double, ctypes.c_double, ctypes.c_double]),
     "cpd_nonrigid_step": (ctypes.c_int, [ctypes.c_void_p, _c_dp]),
     "cpd_nonrigid_get": (ctypes.c_int, [ctypes.c_void_p, _c_dp, _c_dp]),
@@ -148,6 +155,7 @@ class Handle(object):
         check(self._lib.cpd_create(ctypes.byref(self._h), device, dim, ctypes.c_void_p(stream) if stream else None))
         self.m = 0
         self.n = 0
+        self.gmmtree_levels = 0
 
     def close(self):
         if getattr(self, "_h", None) is not None and self._h.value:
@@ -312,6 +320,63 @@ class Handle(object):
         check(self._lib.cpd_mstep(self._h, tf_kind, int(bool(update_scale)), dptr(pt1), dptr(p1), dptr(px), float(n_p),
                               ctypes.byref(p)))
         return self._unpack(p)
+
+    # -- GMMTree (3-D handles only)
+    @staticmethod
+    def gmmtree_total(tree_level):
+        """number of nodes of a tree of `tree_level` levels: 8 (8^L - 1) / 7"""
+        return 8 * (8 ** tree_level - 1) // 7
+
+    def gmmtree_build(self, tree_level, lambda_s, lambda_d, leaf_seeds, maxiter=1000):
+        """buildGmmTree on the handle's source from the 8^L leaf seeds (point indices, caller's order); returns the iterations
+        each level ran."""
+        seeds = np.ascontiguousarray(leaf_seeds, dtype=np.int64)
+        if not 1 <= int(tree_level) <= 5:
+            raise ValueError("tree_level must be in 1..5, got %r" % (tree_level,))
+        if seeds.shape != (8 ** int(tree_level),):
+            raise ValueError("leaf_seeds must hold 8^tree_level = %d indices, got shape %s" % (8 ** int(tree_level), seeds.shape))
+        iters = np.zeros(int(tree_level), dtype=np.int32)
+        check(self._lib.cpd_gmmtree_build(self._h, int(tree_level), float(lambda_s), float(lambda_d),
+                                          seeds.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)), int(maxiter),
+                                          iters.ctypes.data_as(ctypes.POINTER(ctypes.c_int))))
+        self.gmmtree_levels = int(tree_level)
+        return iters
+
+    def gmmtree_nodes(self):
+        """(pi (n_total,), mu (n_total, 3), cov (n_total, 3, 3)) of the handle's tree"""
+        total = self.gmmtree_total(self.gmmtree_levels)
+        pi, mu, cov = np.empty(total), np.empty((total, 3)), np.empty((total, 3, 3))
+        check(self._lib.cpd_gmmtree_nodes(self._h, dptr(pi), dptr(mu), dptr(cov)))
+        return pi, mu, cov
+
+    def gmmtree_load(self, tree_level, pi, mu, cov):
+        total = self.gmmtree_total(int(tree_level)) if 1 <= int(tree_level) <= 5 else 0
+        pi = np.ascontiguousarray(pi, dtype=np.float64)
+        mu = np.ascontiguousarray(mu, dtype=np.float64)
+        cov = np.ascontiguousarray(cov, dtype=np.float64)
+        if total and (pi.shape != (total,) or mu.shape != (total, 3) or cov.shape != (total, 3, 3)):
+            raise ValueError("a tree of %d levels has %d nodes: pi (n,), mu (n, 3), cov (n, 3, 3)" % (tree_level, total))
+        check(self._lib.cpd_gmmtree_load(self._h, int(tree_level), dptr(pi), dptr(mu), dptr(cov)))
+        self.gmmtree_levels = int(tree_level)
+
+    def gmmtree_assign(self):
+        """the node each source point was assigned to in the last E-step of the build (caller's order)"""
+        out = np.empty(self.m, dtype=np.int32)
+        check(self._lib.cpd_gmmtree_assign(self._h, out.ctypes.data_as(ctypes.POINTER(ctypes.c_int32))))
+        return out
+
+    def gmmtree_estep(self, rot, t, lambda_c):
+        """moments (n_total, 13) -- m0, m1 (3), m2 (3 x 3) -- of the handle's target moved by rot x + t"""
+        r = np.ascontiguousarray(rot, dtype=np.float64).reshape(9)
+        tt = np.ascontiguousarray(t, dtype=np.float64).reshape(3)
+        out = np.empty((self.gmmtree_total(self.gmmtree_levels), 13))
+        check(self._lib.cpd_gmmtree_estep(self._h, dptr(r), dptr(tt), float(lambda_c), dptr(out)))
+        return out
+
+    def gmmtree_times(self):
+        lv, es = (ctypes.c_float * 5)(), ctypes.c_float()
+        check(self._lib.cpd_gmmtree_times(self._h, lv, ctypes.byref(es)))
+        return {"level_ms": list(lv), "estep_ms": es.value}
 
     # -- non-rigid (dense G on the device)
     def nonrigid_begin(self, beta, lmd, sigma2, w):

@@ -6,6 +6,7 @@
 #include "lowrank.cuh"
 #include "gram_i8.cuh"
 #include "bcpd.cuh"
+#include "gmmtree.cuh"
 
 #include <cub/device/device_radix_sort.cuh>
 #ifdef CPD_HOST_EMU
@@ -233,6 +234,20 @@ struct cpd_ctx {
     int64_t* d_bc_lr_ipiv = nullptr;
     long long bc_lr_m = 0;
     int bc_lr_k = 0;
+    // GMMTree (host_gmmtree.inl, gmmtree.cuh): the tree (13 doubles per node) and its prepared form (16), per-point work arrays
+    // sized for gt_cap points (coordinates, sorted coordinates, 8 gammas, sort keys / values in and out, argmax), the run bounds
+    // of the keys, the chunk partials, the moments of a registration E-step and scratch
+    int gt_levels = 0;                    // > 0: a tree is installed (cpd_gmmtree_build / cpd_gmmtree_load)
+    long long gt_total = 0, gt_cap = 0, gt_m = 0;   // nodes, point capacity, source count of the last build (0: loaded)
+    size_t gt_part_cap = 0, gt_sort_cap = 0;
+    double *d_gt_nodes = nullptr, *d_gt_prep = nullptr, *d_gt_pts = nullptr, *d_gt_spts = nullptr, *d_gt_g = nullptr,
+           *d_gt_part = nullptr, *d_gt_mom = nullptr, *d_gt_scr = nullptr;
+    unsigned *d_gt_keys = nullptr, *d_gt_keys2 = nullptr;
+    int *d_gt_idx = nullptr, *d_gt_idx2 = nullptr, *d_gt_cur = nullptr, *d_gt_start = nullptr, *d_gt_end = nullptr, *d_gt_asg = nullptr;
+    long long* d_gt_seeds = nullptr;
+    void* d_gt_sort = nullptr;
+    cudaEvent_t gt_ev[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+    float gt_ms[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};   // build ms per level (up to 5), ms of the last registration E-step
     // correspondence priors of ConstrainedNonRigidCPD
     double *d_wgt = nullptr, *d_p1t = nullptr, *d_pxt = nullptr;
     long long prior_m = 0;
@@ -700,6 +715,10 @@ extern "C" void cpd_destroy(cpd_ctx* h) {
                    h->d_bc_ipiv, h->d_bc_info, h->d_bc_sys, h->d_bc_C, h->d_bc_CQ, h->d_bc_rt, h->d_bc_w, h->d_bc_lr_ipiv};
     for (void* p : bcp) if (p) cudaFree(p);
     for (cudaEvent_t e : h->bc_ev) if (e) cudaEventDestroy(e);
+    void* gtp[] = {h->d_gt_nodes, h->d_gt_prep, h->d_gt_pts, h->d_gt_spts, h->d_gt_g, h->d_gt_part, h->d_gt_mom, h->d_gt_scr, h->d_gt_keys,
+                   h->d_gt_keys2, h->d_gt_idx, h->d_gt_idx2, h->d_gt_cur, h->d_gt_start, h->d_gt_end, h->d_gt_asg, h->d_gt_seeds, h->d_gt_sort};
+    for (void* p : gtp) if (p) cudaFree(p);
+    for (cudaEvent_t e : h->gt_ev) if (e) cudaEventDestroy(e);
     if (h->h_work) free(h->h_work);
     if (h->sol_params && g_sol.DestroyParams) g_sol.DestroyParams(h->sol_params);
     if (h->sol && g_sol.Destroy) g_sol.Destroy(h->sol);
@@ -1094,9 +1113,10 @@ extern "C" int cpd_mstep(cpd_ctx* h, int tf_kind, int update_scale, const double
     return read_params(h, out);
 }
 
-// The remaining entry points live in five .inl files of this same translation unit:
+// The remaining entry points live in six .inl files of this same translation unit:
 #include "host_nonrigid.inl"     // cpd_nonrigid_* (dense G, low-rank factors, priors)
 #include "host_bcpd.inl"         // cpd_bcpd_begin / step / get, cpd_bcpd_step_times (the BCPD loop on the device)
+#include "host_gmmtree.inl"      // cpd_gmmtree_* (the GMMTree build and registration E-step)
 #include "host_stateless.inl"    // cpd_rbf_kernel, cpd_imq_kernel, cpd_gauss_transform, cpd_squared_kernel_sum
 #include "host_multi.inl"        // cpd_comm_*, cpd_p2p_*
 #include "host_measure.inl"      // cpd_timer_*, cpd_event_*, cpd_stage_times, cpd_flush_l2, cpd_microbench
