@@ -221,6 +221,29 @@ int cpd_imq_kernel(int device, const double* x, int64_t nx, const double* y, int
 int cpd_gauss_transform(int device, const double* source, int64_t m, const double* target, int64_t n, int dim, double h,
                         const double* weights, int k, double* out);
 
+/* GMMReg (probreg/l2dist_regs.py, cost_functions.py, features.py; csrc/l2dist.cuh), FP64, every reduction in a fixed order
+ * (bit-identical runs on one device).
+ * cpd_gmm_fit: features.GMM's sklearn GaussianMixture(k, covariance_type="spherical", init_params="random_from_data",
+ * reg_covar, tol, max_iter, n_init=1).fit on the handle's source (2-D or 3-D).  seeds: k distinct point indices (caller's order)
+ * where the one-hot initial responsibilities sit; the initial weights are nk / N, unnormalised, as sklearn leaves them.  Each
+ * iteration: E-step (per-point log-sum-exp, lower bound = its mean), M-step (weights nk / sum nk), then the stop test
+ * |lb - lb_prev| < tol.  The pair arithmetic runs in the handle's centred frame; the M-step forms sklearn's parameters in the
+ * caller's frame in residual form (no avg_X2 - 2 avg_X mu + mu^2 cancellation).  Outputs (any may be NULL): weights (k), means
+ * (k x D, caller's frame), variances (k), n_iter, lower_bounds (max_iter doubles, the first n_iter written).  Refused with
+ * CPD_ERR_ARG: k outside 1..m, a seed outside 0..m-1 or repeated, reg_covar < 0 or non-finite, NaN tol, max_iter < 1, a
+ * non-finite source; with CPD_ERR_STATE: no source.
+ * cpd_l2_dist: compute_l2_dist (cost_functions.py:33-41) without a handle, by direct FP64 pair sums (the reference's Gauss
+ * transform is a float32 IFGT): with z = (2 pi sigma^2)^(D/2) and e_ij = exp(-|mu_s,i - mu_t,j|^2 / (2 sigma^2)),
+ * f = -sum_i phi_s,i sum_j (phi_t,j / z) e_ij and g_i = phi_s,i sum_j (phi_t,j / z) e_ij (mu_s,i - mu_t,j) / (2 sigma^2)
+ * (g: ns x D).  Refused: dim not 2 or 3, an empty mixture, sigma <= 0 or non-finite, a non-finite mean or weight.
+ * cpd_tps_kernel: _math.tps_kernel_2d / _3d (cc/math_utils.cc:21-30), float32 like the reference: 2-D r^2 log r (0 where
+ * r^2 <= 1e-9; the log of the float32 r is taken in FP64 and rounded once), 3-D -r.  out: nx x ny.                          */
+int cpd_gmm_fit(cpd_ctx* h, int k, const int64_t* seeds, double reg_covar, double tol, int max_iter, double* weights, double* means,
+                double* variances, int* n_iter, double* lower_bounds);
+int cpd_l2_dist(int device, const double* mu_s, int64_t ns, const double* phi_s, const double* mu_t, int64_t nt, const double* phi_t,
+                int dim, double sigma, double* f, double* g);
+int cpd_tps_kernel(int device, const double* x, int64_t nx, const double* y, int64_t ny, int dim, float* out);
+
 /* math_utils.squared_kernel_sum on two host clouds without a handle.                    */
 int cpd_squared_kernel_sum(int device, const double* x, int64_t nx, const double* y, int64_t ny,
                            int dim, double* out);

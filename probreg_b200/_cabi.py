@@ -73,6 +73,11 @@ _PROTOS = {
                                       ctypes.c_double, _c_fp]),
     "cpd_gauss_transform": (ctypes.c_int, [ctypes.c_int, _c_dp, ctypes.c_int64, _c_dp, ctypes.c_int64, ctypes.c_int, ctypes.c_double,
                                            _c_dp, ctypes.c_int, _c_dp]),
+    "cpd_gmm_fit": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.POINTER(ctypes.c_int64), ctypes.c_double, ctypes.c_double,
+                                   ctypes.c_int, _c_dp, _c_dp, _c_dp, ctypes.POINTER(ctypes.c_int), _c_dp]),
+    "cpd_l2_dist": (ctypes.c_int, [ctypes.c_int, _c_dp, ctypes.c_int64, _c_dp, _c_dp, ctypes.c_int64, _c_dp, ctypes.c_int,
+                                   ctypes.c_double, _c_dp, _c_dp]),
+    "cpd_tps_kernel": (ctypes.c_int, [ctypes.c_int, _c_dp, ctypes.c_int64, _c_dp, ctypes.c_int64, ctypes.c_int, _c_fp]),
     "cpd_squared_kernel_sum": (ctypes.c_int, [ctypes.c_int, _c_dp, ctypes.c_int64, _c_dp, ctypes.c_int64, ctypes.c_int, _c_dp]),
     "cpd_comm_unique_id": (ctypes.c_int, [ctypes.c_char_p]),
     "cpd_comm_create": (ctypes.c_int, [ctypes.POINTER(ctypes.c_void_p), ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_char_p]),
@@ -378,6 +383,21 @@ class Handle(object):
         check(self._lib.cpd_gmmtree_times(self._h, lv, ctypes.byref(es)))
         return {"level_ms": list(lv), "estep_ms": es.value}
 
+    # -- GMMReg: the spherical GMM fit of the source
+    def gmm_fit(self, n_components, seeds, reg_covar=1e-6, tol=1e-3, max_iter=100):
+        """features.GMM's spherical GaussianMixture fit of the handle's source from one-hot responsibilities at `seeds` (distinct
+        point indices, caller's order); returns (weights (K,), means (K, D), variances (K,), n_iter, lower bound per iteration)."""
+        sd = np.ascontiguousarray(seeds, dtype=np.int64)
+        k = int(n_components)
+        if sd.shape != (k,):
+            raise ValueError("seeds must hold n_components = %d indices, got shape %s" % (k, sd.shape))
+        w, mu, var = np.empty(k), np.empty((k, self.dim)), np.empty(k)
+        lb = np.empty(max(int(max_iter), 1))
+        it = ctypes.c_int()
+        check(self._lib.cpd_gmm_fit(self._h, k, sd.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)), float(reg_covar), float(tol),
+                                    int(max_iter), dptr(w), dptr(mu), dptr(var), ctypes.byref(it), dptr(lb)))
+        return w, mu, var, it.value, lb[: it.value]
+
     # -- non-rigid (dense G on the device)
     def nonrigid_begin(self, beta, lmd, sigma2, w):
         check(self._lib.cpd_nonrigid_begin(self._h, float(beta), float(lmd), float(sigma2), float(w)))
@@ -517,6 +537,19 @@ def plan_work(ntiles, nunits, slots, last_tile_cost=1.0):
     check(lib().cpd_plan_work(ntiles, nunits, slots, float(last_tile_cost), buf.ctypes.data_as(ctypes.POINTER(ctypes.c_int)), n.value,
                               ctypes.byref(n), ctypes.byref(mx)))
     return buf, mx.value
+
+
+def l2_dist(mu_source, phi_source, mu_target, phi_target, sigma, device=0):
+    """(f, g) of cost_functions.compute_l2_dist by direct FP64 sums on the device (cpd_l2_dist); g: (n_source, D)."""
+    ms, mt = as_cloud(mu_source), as_cloud(mu_target)
+    ps, pt = np.ascontiguousarray(phi_source, dtype=np.float64), np.ascontiguousarray(phi_target, dtype=np.float64)
+    if ms.shape[1] != mt.shape[1] or ps.shape != (ms.shape[0],) or pt.shape != (mt.shape[0],):
+        raise ValueError("mixture shapes do not match: means %s / %s, weights %s / %s" % (ms.shape, mt.shape, ps.shape, pt.shape))
+    f = ctypes.c_double()
+    g = np.empty(ms.shape)
+    check(lib().cpd_l2_dist(device, dptr(ms), ms.shape[0], dptr(ps), dptr(mt), mt.shape[0], dptr(pt), ms.shape[1], float(sigma),
+                            ctypes.byref(f), dptr(g)))
+    return f.value, g
 
 
 def comm_create(device, world_size, rank, uid):

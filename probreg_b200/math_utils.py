@@ -47,3 +47,16 @@ def inverse_multiquadric_kernel(x, y, c=1.0, device=0):
 def compute_rmse(source, target_tree):
     """probreg/math_utils.py:32-33: mean nearest-neighbour distance of ``source`` in a scipy cKDTree of the target."""
     return float(np.sum(target_tree.query(source)[0]) / source.shape[0])
+
+
+def tps_kernel(x, y, device=0):
+    """probreg/math_utils.py:40-47 -> ``_math.tps_kernel_2d`` / ``_3d`` (cc/math_utils.cc:21-30), float32, on the device
+    (cpd_tps_kernel): 2-D r^2 log r (0 where r^2 <= 1e-9), 3-D -r."""
+    xa, ya = _cabi.as_cloud(x), _cabi.as_cloud(y)
+    assert xa.shape[1] == ya.shape[1], "x and y must have same dimensions."
+    if xa.shape[1] not in (2, 3):
+        raise ValueError("Invalid dimension of x: %d." % xa.shape[1])
+    out = np.empty((xa.shape[0], ya.shape[0]), dtype=np.float32)
+    _cabi.check(_cabi.lib().cpd_tps_kernel(device, _cabi.dptr(xa), xa.shape[0], _cabi.dptr(ya), ya.shape[0], xa.shape[1],
+                                           out.ctypes.data_as(ctypes.POINTER(ctypes.c_float))))
+    return out

@@ -127,3 +127,39 @@ class CombinedTransformation(Transformation):
 
     def _transform(self, points):
         return self.rigid_trans._transform(points + self.v)
+
+
+class TPSTransformation(Transformation):
+    """Thin-plate spline x -> [1, x, U(x) P] [a; v] (transformation.py:124-160): a ((D + 1) x D) the affine part, v
+    ((n - D - 1) x D) the warp on the null space P of [1, control_pts], U the TPS kernel (math_utils.tps_kernel, float32 on the
+    device) against the n control points."""
+
+    def __init__(self, a, v, control_pts, kernel=mu.tps_kernel):
+        super(TPSTransformation, self).__init__()
+        self.a = a
+        self.v = v
+        self.control_pts = control_pts
+        self._kernel = kernel
+
+    def prepare(self, landmarks):
+        """(basis (m x (n + 1)), kernel ((n - D - 1) x (n - D - 1))) of `landmarks`: they depend on the landmarks and the control
+        points only, not on a or v."""
+        control_pts = self.control_pts
+        m, d = landmarks.shape
+        n, _ = control_pts.shape
+        pm = np.c_[np.ones((m, 1)), landmarks]
+        pn = np.c_[np.ones((n, 1)), control_pts]
+        u, _, _ = np.linalg.svd(pn)
+        pp = u[:, d + 1:]
+        kk = self._kernel(control_pts, control_pts)
+        uu = self._kernel(landmarks, control_pts)
+        basis = np.c_[pm, np.dot(uu, pp)]
+        kernel = np.dot(pp.T, np.dot(kk, pp))
+        return basis, kernel
+
+    def transform_basis(self, basis):
+        return np.dot(basis, np.r_[self.a, self.v])
+
+    def _transform(self, points):
+        basis, _ = self.prepare(points)
+        return self.transform_basis(basis)
