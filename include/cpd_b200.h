@@ -244,6 +244,19 @@ int cpd_l2_dist(int device, const double* mu_s, int64_t ns, const double* phi_s,
                 int dim, double sigma, double* f, double* g);
 int cpd_tps_kernel(int device, const double* x, int64_t nx, const double* y, int64_t ny, int dim, float* out);
 
+/* SVR (probreg/l2dist_regs.py RigidSVR / TPSSVR, features.py OneClassSVM; csrc/ocsvm.cuh), without a handle.
+ * cpd_ocsvm_fit: sklearn's OneClassSVM(kernel="rbf", nu, gamma, tol).fit on x (n x dim, row-major), the one-class dual
+ * min 1/2 a^T Q a subject to 0 <= a_i <= 1, sum a = nu n, Q_ij = exp(-gamma |x_i - x_j|^2), by libsvm's SMO with second-order
+ * working-set selection and no shrinking (where measured, sklearn's shrinking gives the same a).  sklearn's path is kept: its
+ * sample-weighted start, the kernel on the raw coordinates in the caller's order rounded to float32 (libsvm's Qfloat), ties
+ * to the larger index, its clipped two-variable step.  FP64 otherwise, every reduction in a fixed order (bit-identical runs on
+ * one device).  Outputs: alpha (n, every point; the support is alpha > 0), rho (libsvm's; sklearn's intercept_ = -rho; +inf
+ * when every alpha is 1, which sklearn refuses), n_iter (updates made; n_iter = max_iter means the cap was reached and alpha
+ * is the current iterate; libsvm's cap is max(10^7, 100 n)).  Refused with CPD_ERR_ARG: dim not 2 or 3, n < 1, nu outside
+ * (0, 1], gamma <= 0 or non-finite, tol <= 0 or NaN, max_iter < 1, a non-finite coordinate.                                 */
+int cpd_ocsvm_fit(int device, const double* x, int64_t n, int dim, double nu, double gamma, double tol, int64_t max_iter, double* alpha,
+                  double* rho, int64_t* n_iter);
+
 /* math_utils.squared_kernel_sum on two host clouds without a handle.                    */
 int cpd_squared_kernel_sum(int device, const double* x, int64_t nx, const double* y, int64_t ny,
                            int dim, double* out);

@@ -78,6 +78,8 @@ _PROTOS = {
     "cpd_l2_dist": (ctypes.c_int, [ctypes.c_int, _c_dp, ctypes.c_int64, _c_dp, _c_dp, ctypes.c_int64, _c_dp, ctypes.c_int,
                                    ctypes.c_double, _c_dp, _c_dp]),
     "cpd_tps_kernel": (ctypes.c_int, [ctypes.c_int, _c_dp, ctypes.c_int64, _c_dp, ctypes.c_int64, ctypes.c_int, _c_fp]),
+    "cpd_ocsvm_fit": (ctypes.c_int, [ctypes.c_int, _c_dp, ctypes.c_int64, ctypes.c_int, ctypes.c_double, ctypes.c_double, ctypes.c_double,
+                                     ctypes.c_int64, _c_dp, _c_dp, ctypes.POINTER(ctypes.c_int64)]),
     "cpd_squared_kernel_sum": (ctypes.c_int, [ctypes.c_int, _c_dp, ctypes.c_int64, _c_dp, ctypes.c_int64, ctypes.c_int, _c_dp]),
     "cpd_comm_unique_id": (ctypes.c_int, [ctypes.c_char_p]),
     "cpd_comm_create": (ctypes.c_int, [ctypes.POINTER(ctypes.c_void_p), ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_char_p]),
@@ -550,6 +552,19 @@ def l2_dist(mu_source, phi_source, mu_target, phi_target, sigma, device=0):
     check(lib().cpd_l2_dist(device, dptr(ms), ms.shape[0], dptr(ps), dptr(mt), mt.shape[0], dptr(pt), ms.shape[1], float(sigma),
                             ctypes.byref(f), dptr(g)))
     return f.value, g
+
+
+def ocsvm_fit(x, nu, gamma, tol=1e-3, max_iter=None, device=0):
+    """(alpha (every point), rho, n_iter) of sklearn's OneClassSVM(kernel="rbf", nu, gamma, tol).fit on the device (cpd_ocsvm_fit);
+    max_iter None: libsvm's cap max(10^7, 100 n)."""
+    xa = as_cloud(x)
+    n = xa.shape[0]
+    max_iter = max(10_000_000, 100 * n) if max_iter is None else int(max_iter)
+    alpha = np.empty(n)
+    rho, it = ctypes.c_double(), ctypes.c_int64()
+    check(lib().cpd_ocsvm_fit(device, dptr(xa), n, xa.shape[1], float(nu), float(gamma), float(tol), max_iter, dptr(alpha),
+                              ctypes.byref(rho), ctypes.byref(it)))
+    return alpha, rho.value, it.value
 
 
 def comm_create(device, world_size, rank, uid):

@@ -8,6 +8,7 @@
 #include "bcpd.cuh"
 #include "gmmtree.cuh"
 #include "l2dist.cuh"
+#include "ocsvm.cuh"
 
 #include <cub/device/device_radix_sort.cuh>
 #ifdef CPD_HOST_EMU
@@ -1120,5 +1121,6 @@ extern "C" int cpd_mstep(cpd_ctx* h, int tf_kind, int update_scale, const double
 #include "host_gmmtree.inl"      // cpd_gmmtree_* (the GMMTree build and registration E-step)
 #include "host_stateless.inl"    // cpd_rbf_kernel, cpd_imq_kernel, cpd_gauss_transform, cpd_squared_kernel_sum
 #include "host_l2dist.inl"       // cpd_gmm_fit, cpd_l2_dist, cpd_tps_kernel (GMMReg)
+#include "host_ocsvm.inl"        // cpd_ocsvm_fit (the one-class SVM of SVR)
 #include "host_multi.inl"        // cpd_comm_*, cpd_p2p_*
 #include "host_measure.inl"      // cpd_timer_*, cpd_event_*, cpd_stage_times, cpd_flush_l2, cpd_microbench

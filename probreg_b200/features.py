@@ -6,9 +6,15 @@ fit, run on the device (``cpd_gmm_fit``: FP64 EM, fixed-order reductions, bit-id
 Departure from the reference, on purpose: the fit starts from ``init_params="random_from_data"`` seeded by ``seed`` -- the K
 points ``np.random.RandomState(seed).choice(N, K, replace=False)``, exactly sklearn's draw for ``random_state=seed`` -- where the
 reference runs sklearn's default, an unseeded k-means initialisation.  The device has no k-means, and a seeded start makes every
-fit reproducible.  FPFH and the one-class SVM of the reference are not provided.
+fit reproducible.
+
+``OneClassSVM`` summarises a cloud by the support vectors of sklearn's ``OneClassSVM(kernel="rbf", nu, gamma)`` fit, run on the
+device (``cpd_ocsvm_fit``): libsvm's SMO on sklearn's path, so the same support vectors and weights as the reference's fit.  It has
+no shrinking (where measured, sklearn's shrinking gives the same weights) and keeps libsvm's float32 rounding of the kernel values
+on purpose, since the badly conditioned dual would otherwise end on other weights.  FPFH is not provided.
 """
 import abc
+import warnings
 
 import numpy as np
 
@@ -64,3 +70,51 @@ class GMM(Feature):
             h.close()
         self.weights_, self.means_, self.covariances_, self.n_iter_, self.lower_bounds_ = w, mu, var, it, lb
         return mu, w
+
+
+class ConvergenceWarning(UserWarning):
+    """the one-class SVM fit reached max_iter before its stop test held (sklearn warns with its own ConvergenceWarning)"""
+
+
+class OneClassSVM(Feature):
+    """Feature points extraction using One class SVM
+
+    dim -- dimension of the points; sigma -- width of the Gaussians the support vectors become (weights alpha (2 pi sigma^2)^(D/2));
+    gamma -- coefficient of the RBF kernel; nu -- sklearn's nu, in (0, 1]; delta -- annealing factor of gamma.  Extensions over the
+    reference: device (CUDA ordinal), tol (of the stop test), max_iter (SMO iterations; None: libsvm's max(10^7, 100 N)).  After
+    ``compute``, as sklearn names them: ``support_``, ``support_vectors_``, ``dual_coef_`` (1 x nSV), ``intercept_`` (-rho),
+    ``offset_`` (rho) and ``n_iter_``.
+    """
+
+    def __init__(self, dim, sigma, gamma=0.5, nu=0.05, delta=10.0, device=0, tol=1.0e-3, max_iter=None):
+        self._dim = dim
+        self._sigma = sigma
+        self._gamma = gamma
+        self._nu = nu
+        self._delta = delta
+        self._device = device
+        self._tol = tol
+        self._max_iter = max_iter
+
+    def init(self):
+        pass
+
+    def compute(self, data):
+        x = _cabi.as_cloud(data, self._dim)
+        max_iter = max(10_000_000, 100 * len(x)) if self._max_iter is None else self._max_iter
+        alpha, rho, it = _cabi.ocsvm_fit(x, self._nu, self._gamma, self._tol, max_iter, self._device)
+        if not np.isfinite(rho):
+            raise ValueError("The dual coefficients or intercepts are not finite (every alpha is at its bound 1: nu = %g)" % self._nu)
+        if it >= max_iter:
+            warnings.warn("the one-class SVM fit stopped at max_iter = %d before converging" % max_iter, ConvergenceWarning)
+        self.support_ = np.nonzero(alpha > 0.0)[0].astype(np.int32)
+        self.support_vectors_ = x[self.support_]
+        self.dual_coef_ = alpha[self.support_][None, :]
+        self.intercept_ = np.array([-rho])
+        self.offset_ = np.array([rho])
+        self.n_iter_ = it
+        z = np.power(2.0 * np.pi * self._sigma ** 2, self._dim * 0.5)
+        return self.support_vectors_, self.dual_coef_[0] * z
+
+    def annealing(self):
+        self._gamma *= self._delta

@@ -10,7 +10,11 @@ Departures from the reference, on purpose:
   * the Gauss transforms of the L2 distance are exact FP64 sums, not a float32 IFGT;
   * ``TPSGMMReg`` fits the source once, in the constructor, and its means are both the control points and the source mixture of
     every outer iteration: the reference fits it again each time, which with a seeded start gives the same mixture.
-The support-vector registrations (``RigidSVR``, ``TPSSVR``, ``registration_svr``) are not provided.
+
+Support vector registration (``RigidSVR``, ``TPSSVR``, ``registration_svr``) summarises each cloud by the support vectors of a
+one-class SVM (``features.OneClassSVM``: the SMO fit on the device, ``cpd_ocsvm_fit``, on sklearn's path) and minimises the same
+L2 distance.  The kernel's gamma is annealed by x10 per outer iteration, so ``TPSSVR`` fits the source again in every outer
+iteration after the first; its control points are the support vectors of the constructor's fit, as in the reference.
 """
 import logging
 
@@ -108,6 +112,41 @@ class TPSGMMReg(L2DistRegistration):
         return self._src_features
 
 
+class RigidSVR(L2DistRegistration):
+    """Rigid support vector registration.  Extension over the reference: device (CUDA ordinal)."""
+
+    def __init__(self, source, sigma=1.0, delta=0.9, gamma=0.5, nu=0.1, use_estimated_sigma=True, device=0):
+        super(RigidSVR, self).__init__(source, ft.OneClassSVM(source.shape[1], sigma, gamma, nu, device=device),
+                                       cf.RigidCostFunction(device), sigma, delta, use_estimated_sigma)
+
+    def _estimate_sigma(self, data):
+        super(RigidSVR, self)._estimate_sigma(data)
+        self._feature_gen._sigma = self._sigma
+        self._feature_gen._gamma = 1.0 / (2.0 * np.square(self._sigma))
+
+
+class TPSSVR(L2DistRegistration):
+    """Thin-plate-spline support vector registration: the support vectors of the source's first fit are the spline's control
+    points.  Extension over the reference: device."""
+
+    def __init__(self, source, sigma=1.0, delta=0.9, gamma=0.5, nu=0.1, alpha=1.0, beta=0.1, use_estimated_sigma=True, device=0):
+        super(TPSSVR, self).__init__(source, ft.OneClassSVM(source.shape[1], sigma, gamma, nu, device=device),
+                                     cf.TPSCostFunction([], alpha, beta, device), sigma, delta, use_estimated_sigma)
+        self._feature_gen.init()
+        self._first_features = self._feature_gen.compute(source)
+        self._cost_fn._control_pts = self._first_features[0]
+
+    def _estimate_sigma(self, data):
+        super(TPSSVR, self)._estimate_sigma(data)
+        self._feature_gen._sigma = self._sigma
+        self._feature_gen._gamma = 1.0 / (2.0 * np.square(self._sigma))
+
+    def _source_features(self):
+        # the constructor's fit is the first outer iteration's (same gamma); gamma anneals after it, so later ones fit again
+        feats, self._first_features = self._first_features, None
+        return feats if feats is not None else self._feature_gen.compute(self._source)
+
+
 def registration_gmmreg(source, target, tf_type_name="rigid", callbacks=[], **kargs):
     """GMMReg of source to target; tf_type_name 'rigid' or 'nonrigid' (TPS); callbacks get the transformation at every BFGS
     iteration; keyword args go to RigidGMMReg / TPSGMMReg.  Returns the transformation from source to target."""
@@ -120,3 +159,19 @@ def registration_gmmreg(source, target, tf_type_name="rigid", callbacks=[], **ka
         raise ValueError("Unknown transform type %s" % tf_type_name)
     gmmreg.set_callbacks(callbacks)
     return gmmreg.registration(cv(target))
+
+
+def registration_svr(source, target, tf_type_name="rigid", maxiter=1, tol=1.0e-3, opt_maxiter=50, opt_tol=1.0e-3, callbacks=[],
+                     **kwargs):
+    """Support vector registration of source to target; tf_type_name 'rigid' or 'nonrigid' (TPS); maxiter / tol: the outer loop,
+    opt_maxiter / opt_tol: BFGS; callbacks get the transformation at every BFGS iteration; keyword args go to RigidSVR / TPSSVR.
+    Returns the transformation from source to target."""
+    cv = lambda x: np.asarray(x.points if hasattr(x, "points") else x)  # noqa: E731 (open3d clouds pass their points)
+    if tf_type_name == "rigid":
+        svr = RigidSVR(cv(source), **kwargs)
+    elif tf_type_name == "nonrigid":
+        svr = TPSSVR(cv(source), **kwargs)
+    else:
+        raise ValueError("Unknown transform type %s" % tf_type_name)
+    svr.set_callbacks(callbacks)
+    return svr.registration(cv(target), maxiter, tol, opt_maxiter, opt_tol)
