@@ -163,7 +163,7 @@ struct cpd_ctx {
     long long m = 0, mpad = 0, n = 0, npad = 0, n_global = 0;
     double *d_yc = nullptr, *d_ts = nullptr, *d_xc = nullptr, *d_raw = nullptr;
     size_t raw_cap = 0;
-    float4 *d_srcP = nullptr, *d_srcJ = nullptr, *d_tgtP = nullptr, *d_tgtQ = nullptr;
+    float4 *d_srcP = nullptr, *d_tgtP = nullptr, *d_tgtQ = nullptr;
     P1Part* d_part1 = nullptr;
     double* d_part2 = nullptr;
     size_t part1_cap = 0, part2_cap = 0;
@@ -559,7 +559,7 @@ int launch_estep(cpd_ctx* h, const double* d_sigma2, const double* d_w, const do
     const long long cover = std::max(h->mpad, h->n);
     mark(h, 0);
     pack_kernel<<<blocks_for(cover), THREADS, 0, h->stream>>>(h->d_state, d_sigma2, h->d_yc, d_ts, h->d_xc, h->m, h->mpad,
-                                                              h->n, h->d_srcP, h->d_srcJ, h->d_tgtP);
+                                                              h->n, h->d_srcP, h->d_tgtP);
     mark(h, 1);
     const bool cull = h->cull_on && h->cull_active;
     const int nst1 = (int)(h->mpad / P1_STAGE);
@@ -574,10 +574,10 @@ int launch_estep(cpd_ctx* h, const double* d_sigma2, const double* d_w, const do
     }
     const bool wgt = h->wgt_on;
     if (wgt) {
-        weight_patch_kernel<<<blocks_for(h->m), THREADS, 0, h->stream>>>(h->d_la, h->m, h->d_srcP, h->d_srcJ);
+        weight_patch_kernel<<<blocks_for(h->m), THREADS, 0, h->stream>>>(h->d_la, h->m, h->d_srcP);
         h->launches += 1;
     }
-#define CPD_PASS1(C, W) pass1_kernel<C, W><<<h->g1, THREADS, PASS1_SMEM, h->stream>>>(h->d_tgtP, (int)h->n, h->d_srcJ, h->d_work1, h->d_part1, h->d_sbox, nst1, (C) ? h->d_ssub : nullptr)
+#define CPD_PASS1(C, W) pass1_kernel<C, W><<<h->g1, THREADS, PASS1_SMEM, h->stream>>>(h->d_tgtP, (int)h->n, h->d_srcP, h->d_work1, h->d_part1, h->d_sbox, nst1, (C) ? h->d_ssub : nullptr)
     if (cull) { if (wgt) CPD_PASS1(true, true); else CPD_PASS1(true, false); }
     else { if (wgt) CPD_PASS1(false, true); else CPD_PASS1(false, false); }
 #undef CPD_PASS1
@@ -727,7 +727,7 @@ extern "C" void cpd_destroy(cpd_ctx* h) {
     for (int r = 0; r < P2P_MAX; ++r) if (h->peer_ptr[r]) cudaIpcCloseMemHandle(h->peer_ptr[r]);
     if (h->d_box) cudaFree(h->d_box);
     if (h->d_p2p) cudaFree(h->d_p2p);
-    void* ptrs[] = {h->d_yc, h->d_ts, h->d_xc, h->d_raw, h->d_srcP, h->d_srcJ, h->d_tgtP, h->d_tgtQ, h->d_part1, h->d_part2, h->d_pt1, h->d_p1,
+    void* ptrs[] = {h->d_yc, h->d_ts, h->d_xc, h->d_raw, h->d_srcP, h->d_tgtP, h->d_tgtQ, h->d_part1, h->d_part2, h->d_pt1, h->d_p1,
                     h->d_pxc, h->d_px, h->d_mom_src, h->d_mom_tgt, h->d_mom, h->d_sums, h->d_state, h->d_flush};
     for (void* p : ptrs) if (p) cudaFree(p);
     if (h->h_pin) cudaFreeHost(h->h_pin);
@@ -758,7 +758,6 @@ extern "C" int cpd_set_source(cpd_ctx* h, const double* source, int64_t m) {
         TRY(dev_alloc(&h->d_yc, (size_t)m * 3));
         TRY(dev_alloc(&h->d_ts, (size_t)m * 3));
         TRY(dev_alloc(&h->d_srcP, (size_t)h->mpad));
-        TRY(dev_alloc(&h->d_srcJ, (size_t)h->mpad * 2));
         TRY(dev_alloc(&h->d_p1, (size_t)m));
         TRY(dev_alloc(&h->d_pxc, (size_t)m * 3));
         TRY(dev_alloc(&h->d_px, (size_t)m * 3));
@@ -786,7 +785,7 @@ extern "C" int cpd_set_target(cpd_ctx* h, const double* target, int64_t n_local,
         h->npad = (n_local + P2_STAGE - 1) / P2_STAGE * P2_STAGE;
         TRY(dev_alloc(&h->d_xc, (size_t)n_local * 3));
         TRY(dev_alloc(&h->d_tgtP, (size_t)n_local));
-        TRY(dev_alloc(&h->d_tgtQ, (size_t)h->npad * 3));
+        TRY(dev_alloc(&h->d_tgtQ, (size_t)h->npad * 2));
         TRY(dev_alloc(&h->d_pt1, (size_t)n_local));
         TRY(dev_alloc(&h->d_perm_tgt, (size_t)n_local));
         TRY(dev_alloc(&h->d_outN, (size_t)n_local));

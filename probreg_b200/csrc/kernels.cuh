@@ -30,7 +30,10 @@
 
 namespace cpd {
 
-// tunables (tools/tune.sh builds variants with -D...; the defaults are not tuned for the H100)
+// tunables (tools/tune.sh builds variants with -D...).  RI1, RI2, THREADS, the stage sizes and the passes' occupancy fix the
+// work decomposition -- which targets a warp holds, so its offset seeds, and where the work plan cuts the FP64 sums -- and with
+// it every rounding of the results, so changing one changes the results' last bits.  On the H100 the pipeline depth
+// (NSTAGE 2 and 4) and 1024- or 2048-record pass-1 stages measured no faster than these values.
 #ifndef CPD_RI1
 #define CPD_RI1 4
 #endif
@@ -59,17 +62,17 @@ constexpr int UNROLL1 = CPD_UNROLL1, UNROLL2 = CPD_UNROLL2;
 constexpr int THREADS = 256;           // threads per CTA in both passes
 constexpr int RI1 = CPD_RI1, RI2 = CPD_RI2;            // i-points held in registers per thread (pass 1 / pass 2)
 constexpr int ITILE1 = THREADS * RI1, ITILE2 = THREADS * RI2;   // i-points per CTA
-constexpr int NPAIR1 = RI1 / 2, NPAIR2 = RI2 / 2;      // i-points are processed in pairs (fsub2 / ffma2 below)
 #ifndef CPD_P1_STAGE
 #define CPD_P1_STAGE 512
 #endif
 #ifndef CPD_P2_STAGE
 #define CPD_P2_STAGE 512
 #endif
-constexpr int P1_STAGE = CPD_P1_STAGE;   // sources per TMA stage in pass 1 (32 B records -> 16 KB); a multiple of 256
-constexpr int P2_STAGE = CPD_P2_STAGE;   // targets per TMA stage in pass 2 (48 B records -> 24 KB); a multiple of 256
+constexpr int P1_STAGE = CPD_P1_STAGE;   // sources per TMA stage in pass 1 (16 B records -> 8 KB); a multiple of 256
+constexpr int P2_STAGE = CPD_P2_STAGE;   // targets per TMA stage in pass 2 (32 B records -> 16 KB); a multiple of 256
 static_assert(P1_STAGE % 256 == 0 && P2_STAGE % 256 == 0 && P1_STAGE >= 256 && P2_STAGE >= 256, "stage sizes are multiples of 256");
-constexpr int P1_REC = 32, P2_REC = 48;    // bytes per streamed j-record (coordinates duplicated for the pair loops)
+// bytes per streamed j-record: pass 1 {x,y,z,la} (srcP itself), pass 2 {x,y,z,-o},{rn,0,0,0} (tgtQ)
+constexpr int P1_REC = 16, P2_REC = 32;
 #ifndef CPD_NSTAGE
 #define CPD_NSTAGE 3
 #endif
@@ -254,7 +257,7 @@ __global__ void __launch_bounds__(THREADS)
 pack_kernel(const DevState* __restrict__ st, const double* __restrict__ sigma2_ptr,
             const double* __restrict__ yc /* m x 3 centred sources */, const double* __restrict__ ts /* explicit transformed sources or null */,
             const double* __restrict__ xc /* n x 3 centred targets */, long long m, long long mpad, long long n,
-            float4* __restrict__ srcP /* i-points of pass 2 */, float4* __restrict__ srcJ /* j-records of pass 1: {x,x,y,y},{z,z,0,0} */,
+            float4* __restrict__ srcP /* {x,y,z,0}: i-points of pass 2 and j-records of pass 1 */,
             float4* __restrict__ tgtP /* i-points of pass 1 */) {
     const long long i = (long long)blockIdx.x * THREADS + threadIdx.x;
     const double sk = sqrt(LOG2E / (2.0 * *sigma2_ptr));
@@ -284,33 +287,25 @@ pack_kernel(const DevState* __restrict__ st, const double* __restrict__ sigma2_p
             o = make_float4(FAR_COORD, FAR_COORD, FAR_COORD, 0.0f);
         }
         srcP[i] = o;
-        srcJ[2 * i] = make_float4(o.x, o.x, o.y, o.y);
-        srcJ[2 * i + 1] = make_float4(o.z, o.z, 0.0f, 0.0f);
     }
     if (i < n) {
         tgtP[i] = make_float4((float)(sk * xc[3 * i]), (float)(sk * xc[3 * i + 1]), (float)(sk * xc[3 * i + 2]), 0.0f);
     }
 }
 
-// Per-source weights of a weighted E-step (BCPD): la_m = -log2(weight_m) - min(...) >= 0 goes into the spare lanes of the
-// records pack_kernel wrote: srcP[m].w (pass 2 i-points) and srcJ[2m+1].zw (pass 1 j-records).  Padding keeps 0.
+// Per-source weights of a weighted E-step (BCPD): la_m = -log2(weight_m) - min(...) >= 0 goes into the spare lane of the
+// record pack_kernel wrote, srcP[m].w (read by both passes).  Padding keeps 0.
 __global__ void __launch_bounds__(THREADS)
-weight_patch_kernel(const float* __restrict__ la, long long m, float4* __restrict__ srcP, float4* __restrict__ srcJ) {
+weight_patch_kernel(const float* __restrict__ la, long long m, float4* __restrict__ srcP) {
     const long long i = (long long)blockIdx.x * THREADS + threadIdx.x;
-    if (i < m) {
-        const float v = la[i];
-        srcP[i].w = v;
-        float4 r = srcJ[2 * i + 1];
-        r.z = v; r.w = v;
-        srcJ[2 * i + 1] = r;
-    }
+    if (i < m) srcP[i].w = la[i];
 }
 
 // ---------------------------------------------------------------------------------------------
 // pass 1: per target n and split:  (o, S, SU) with  sum_m 2^(-u) = S 2^(-o),  sum_m 2^(-u) u = SU 2^(-o)
 // One CTA per work item {target tile, source-stage range, partial slot}; the host chooses the number of stage
 // ranges per tile that minimises the makespan over the resident CTA slots (build_work in cpd_b200.cu).
-// Per two pairs: 8 packed FP32 instructions + 2 MUFU in the common path.
+// Per pair: 8 FP32 instructions + 1 MUFU.EX2 in the common path (tools/sass_pairloop.py counts the group loop as compiled).
 //
 // Lazy log-sum-exp: each target carries an integer-valued offset o (only ever lowered), seeded per warp from
 // the nearest source stage.  A sub-chunk of 64 sources is summed in FP32 with the current o -- groups of 8 from
@@ -368,7 +363,7 @@ stage_omax_kernel(const float4* __restrict__ tgtQ, float* __restrict__ omax) {
     __shared__ float sh[THREADS / 32];
     const int b = blockIdx.x;
     float m = 3.0e38f;
-    for (int i = threadIdx.x; i < P2_STAGE; i += THREADS) m = fminf(m, tgtQ[3 * ((size_t)b * P2_STAGE + i) + 1].z);
+    for (int i = threadIdx.x; i < P2_STAGE; i += THREADS) m = fminf(m, tgtQ[2 * ((size_t)b * P2_STAGE + i)].w);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) m = fminf(m, __shfl_xor_sync(0xffffffffu, m, o));
     if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = m;
@@ -407,21 +402,20 @@ sub_omax_kernel(const float4* __restrict__ tgtQ, int nsub, float* __restrict__ o
     const int b = blockIdx.x * (THREADS / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (b >= nsub) return;
     float m = 3.0e38f;
-    for (int i = lane; i < SUB; i += 32) m = fminf(m, tgtQ[3 * ((size_t)b * SUB + i) + 1].z);
+    for (int i = lane; i < SUB; i += 32) m = fminf(m, tgtQ[2 * ((size_t)b * SUB + i)].w);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) m = fminf(m, __shfl_xor_sync(0xffffffffu, m, o));
     if (lane == 0) omax[b] = -m;
 }
-// bounding box of this warp's packed i-points -> wbox[0..6) (shared, one row per warp)
-template <int NP>
-__device__ __forceinline__ void warp_bbox(const u64 (&ax)[NP], const u64 (&ay)[NP], const u64 (&az)[NP], float* __restrict__ wbox) {
+// bounding box of this warp's i-points -> wbox[0..6) (shared, one row per warp)
+template <int RI>
+__device__ __forceinline__ void warp_bbox(const float (&ax)[RI], const float (&ay)[RI], const float (&az)[RI], float* __restrict__ wbox) {
     float lo[3] = {3.0e38f, 3.0e38f, 3.0e38f}, hi[3] = {-3.0e38f, -3.0e38f, -3.0e38f};
 #pragma unroll
-    for (int p = 0; p < NP; ++p) {
-        const float2 x = unpack2(ax[p]), y = unpack2(ay[p]), z = unpack2(az[p]);
-        lo[0] = fminf(lo[0], fminf(x.x, x.y)); hi[0] = fmaxf(hi[0], fmaxf(x.x, x.y));
-        lo[1] = fminf(lo[1], fminf(y.x, y.y)); hi[1] = fmaxf(hi[1], fmaxf(y.x, y.y));
-        lo[2] = fminf(lo[2], fminf(z.x, z.y)); hi[2] = fmaxf(hi[2], fmaxf(z.x, z.y));
+    for (int r = 0; r < RI; ++r) {
+        lo[0] = fminf(lo[0], ax[r]); hi[0] = fmaxf(hi[0], ax[r]);
+        lo[1] = fminf(lo[1], ay[r]); hi[1] = fmaxf(hi[1], ay[r]);
+        lo[2] = fminf(lo[2], az[r]); hi[2] = fmaxf(hi[2], az[r]);
     }
 #pragma unroll
     for (int a = 0; a < 3; ++a) {
@@ -449,58 +443,59 @@ __device__ __forceinline__ float box_gap2(const float* __restrict__ wbox, const 
 // Why: adding thousands of tiny terms one by one to a partial sum that already holds a dominant term drops
 // them (absorption), a SYSTEMATIC loss that does not average out -- measured -1.2e-6 on sigma2 with a flat
 // 64-term sum, -2e-6 with 128.
-// WGT: every source carries a weight 2^-la (la >= 0) in the spare half of its z-record; t' = u - o + la, added LAST so that
+// WGT: every source carries a weight 2^-la (la >= 0) in the w lane of its record; t' = u - o + la, added LAST so that
 // pass 2 (which adds the same la after the same FMA chain) sees bit-identical exponents (the BCPD E-step, bcpd.py:53-66).
+// Each operation is a round-to-nearest intrinsic, so the compiler cannot contract or reorder what both passes must agree on.
 template <bool WGT>
-__device__ __forceinline__ void pass1_sum(const ulonglong2* __restrict__ q, const u64 (&ax)[NPAIR1], const u64 (&ay)[NPAIR1],
-                                          const u64 (&az)[NPAIR1], const u64 (&no)[NPAIR1], u64 (&Sc)[NPAIR1], u64 (&Uc)[NPAIR1]) {
+__device__ __forceinline__ float pass1_t(const float ax, const float ay, const float az, const float no, const float4 b) {
+    const float dx = __fsub_rn(ax, b.x), dy = __fsub_rn(ay, b.y), dz = __fsub_rn(az, b.z);
+    float t = __fmaf_rn(dz, dz, __fmaf_rn(dy, dy, __fmaf_rn(dx, dx, no)));
+    if (WGT) t = __fadd_rn(t, b.w);
+    return t;
+}
+template <bool WGT>
+__device__ __forceinline__ void pass1_sum(const float4* __restrict__ q, const float (&ax)[RI1], const float (&ay)[RI1],
+                                          const float (&az)[RI1], const float (&no)[RI1], float (&Sc)[RI1], float (&Uc)[RI1]) {
     if (GRP > 0) {
 #pragma unroll 1
         for (int g0 = 0; g0 < SUB; g0 += (GRP > 0 ? GRP : SUB)) {
-            u64 gs[NPAIR1], gu[NPAIR1];
+            float gs[RI1], gu[RI1];
+            // i-point outer, source inner: the same operations as the other nesting, but ptxas then interleaves the EX2s with
+            // the FP32 work more evenly (measured on the H100: 1.3 % less pass-1 time)
 #pragma unroll
-            for (int jj = 0; jj < (GRP > 0 ? GRP : 1); ++jj) {
-                const ulonglong2 bxy = q[2 * (g0 + jj)];
-                const u64 bz = q[2 * (g0 + jj) + 1].x;
-                u64 la = 0ull;
-                if (WGT) la = q[2 * (g0 + jj) + 1].y;
+            for (int r = 0; r < RI1; ++r) {
 #pragma unroll
-                for (int p = 0; p < NPAIR1; ++p) {
-                    const u64 dx = fsub2(ax[p], bxy.x), dy = fsub2(ay[p], bxy.y), dz = fsub2(az[p], bz);
-                    u64 t = ffma2(dx, dx, no[p]);
-                    t = ffma2(dy, dy, t);
-                    t = ffma2(dz, dz, t);
-                    if (WGT) t = fadd2(t, la);
-                    const float2 tt = unpack2(t);
-                    const u64 e = pack2(ex2(-tt.x), ex2(-tt.y));
-                    gs[p] = jj == 0 ? e : fadd2(gs[p], e);
-                    gu[p] = jj == 0 ? fmul2(e, t) : ffma2(e, t, gu[p]);
+                for (int jj = 0; jj < (GRP > 0 ? GRP : 1); ++jj) {
+                    const float t = pass1_t<WGT>(ax[r], ay[r], az[r], no[r], q[g0 + jj]);
+                    const float e = ex2(-t);
+                    gs[r] = jj == 0 ? e : __fadd_rn(gs[r], e);
+                    gu[r] = jj == 0 ? __fmul_rn(e, t) : __fmaf_rn(e, t, gu[r]);
                 }
             }
 #pragma unroll
-            for (int p = 0; p < NPAIR1; ++p) { Sc[p] = fadd2(Sc[p], gs[p]); Uc[p] = fadd2(Uc[p], gu[p]); }
+            for (int r = 0; r < RI1; ++r) { Sc[r] = __fadd_rn(Sc[r], gs[r]); Uc[r] = __fadd_rn(Uc[r], gu[r]); }
         }
     } else {
 #pragma unroll UNROLL1
         for (int jj = 0; jj < SUB; ++jj) {
-            const ulonglong2 bxy = q[2 * jj];
-            const u64 bz = q[2 * jj + 1].x;
-            u64 la = 0ull;
-            if (WGT) la = q[2 * jj + 1].y;
+            const float4 b = q[jj];
 #pragma unroll
-            for (int p = 0; p < NPAIR1; ++p) {
-                const u64 dx = fsub2(ax[p], bxy.x), dy = fsub2(ay[p], bxy.y), dz = fsub2(az[p], bz);
-                u64 t = ffma2(dx, dx, no[p]);
-                t = ffma2(dy, dy, t);
-                t = ffma2(dz, dz, t);
-                if (WGT) t = fadd2(t, la);
-                const float2 tt = unpack2(t);
-                const u64 e = pack2(ex2(-tt.x), ex2(-tt.y));
-                Sc[p] = fadd2(Sc[p], e);
-                Uc[p] = ffma2(e, t, Uc[p]);
+            for (int r = 0; r < RI1; ++r) {
+                const float t = pass1_t<WGT>(ax[r], ay[r], az[r], no[r], b);
+                const float e = ex2(-t);
+                Sc[r] = __fadd_rn(Sc[r], e);
+                Uc[r] = __fmaf_rn(e, t, Uc[r]);
             }
         }
     }
+}
+// u = |a - b|^2 (+ la under WGT) of the offset checks: the seeding sweep and the rebasing slow path of pass 1
+template <bool WGT>
+__device__ __forceinline__ float pass1_u(const float ax, const float ay, const float az, const float4 b) {
+    const float dx = __fsub_rn(ax, b.x), dy = __fsub_rn(ay, b.y), dz = __fsub_rn(az, b.z);
+    float u = __fmaf_rn(dz, dz, __fmaf_rn(dy, dy, __fmul_rn(dx, dx)));
+    if (WGT) u = __fadd_rn(u, b.w);
+    return u;
 }
 
 template <bool CULL, bool WGT>
@@ -533,25 +528,23 @@ pass1_kernel(const float4* __restrict__ ipts, int ni, const float4* __restrict__
     // barriers then count the remaining warps only (warp 0, the TMA issuer, always has i-points); build_work() gives such a tile
     // correspondingly longer items.
     if (itile * ITILE1 + (tid >> 5) * (32 * RI1) >= ni) return;
-    // two packed pairs of targets per thread: pair p = targets (2p, 2p+1) of this thread
-    u64 ax[NPAIR1], ay[NPAIR1], az[NPAIR1], no[NPAIR1];    // no = (-o, -o'): negated integer offsets
+    float ax[RI1], ay[RI1], az[RI1], no[RI1];    // no = -o: negated integer offsets
     double S[RI1], SU[RI1];
 #pragma unroll
-    for (int p = 0; p < NPAIR1; ++p) {
+    for (int r = 0; r < RI1; ++r) {
         // a warp owns 32*RI1 CONSECUTIVE (Z-ordered) targets: compact for the culling test, still coalesced per 32
-        int n0 = itile * ITILE1 + (tid >> 5) * (32 * RI1) + (2 * p) * 32 + (tid & 31), n1 = n0 + 32;
-        n0 = n0 < ni ? n0 : ni - 1;
-        n1 = n1 < ni ? n1 : ni - 1;
-        const float4 p0 = ipts[n0], p1 = ipts[n1];
-        ax[p] = pack2(p0.x, p1.x); ay[p] = pack2(p0.y, p1.y); az[p] = pack2(p0.z, p1.z);
-        no[p] = pack2(-O_INIT, -O_INIT);
+        int n = itile * ITILE1 + (tid >> 5) * (32 * RI1) + r * 32 + (tid & 31);
+        n = n < ni ? n : ni - 1;
+        const float4 p = ipts[n];
+        ax[r] = p.x; ay[r] = p.y; az[r] = p.z;
+        no[r] = -O_INIT;
     }
     // Seed the offsets from the source stage whose bounding box is nearest to this warp's targets (any source
     // gives a valid upper bound of the final offset; a near one gives a tight bound).  With tight seeds the
     // offset slow path below becomes rare even when sigma << extent, and the culling test bites from the first
     // stage on.  Cost: one scan of the stage boxes + one 128-source sweep per warp.
     float* const mybox = wbox[tid >> 5];
-    warp_bbox<NPAIR1>(ax, ay, az, mybox);
+    warp_bbox<RI1>(ax, ay, az, mybox);
     {
         const int lane = tid & 31;
         float best = 3.0e38f;
@@ -566,35 +559,24 @@ pass1_kernel(const float4* __restrict__ ipts, int ni, const float4* __restrict__
             const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
             if (ob < best || (ob == best && oi < bi)) { best = ob; bi = oi; }
         }
-        const ulonglong2* near = reinterpret_cast<const ulonglong2*>(jbytes + (size_t)bi * P1_STAGE_BYTES);
+        const float4* near = jrec + (size_t)bi * P1_STAGE;
         float cm[RI1];
 #pragma unroll
         for (int r = 0; r < RI1; ++r) cm[r] = 3.0e38f;
 #pragma unroll 4
         for (int jj = 0; jj < 128; ++jj) {
-            const ulonglong2 bxy = near[2 * jj];
-            const u64 bz = near[2 * jj + 1].x;
-            u64 la = 0ull;
-            if (WGT) la = near[2 * jj + 1].y;
+            const float4 b = near[jj];
 #pragma unroll
-            for (int p = 0; p < NPAIR1; ++p) {
-                const u64 dx = fsub2(ax[p], bxy.x), dy = fsub2(ay[p], bxy.y), dz = fsub2(az[p], bz);
-                u64 uu = ffma2(dz, dz, ffma2(dy, dy, fmul2(dx, dx)));
-                if (WGT) uu = fadd2(uu, la);
-                const float2 u = unpack2(uu);
-                cm[2 * p] = fminf(cm[2 * p], u.x);
-                cm[2 * p + 1] = fminf(cm[2 * p + 1], u.y);
-            }
+            for (int r = 0; r < RI1; ++r) cm[r] = fminf(cm[r], pass1_u<WGT>(ax[r], ay[r], az[r], b));
         }
 #pragma unroll
-        for (int p = 0; p < NPAIR1; ++p)
-            no[p] = pack2(-fminf(O_INIT, floorf(cm[2 * p])), -fminf(O_INIT, floorf(cm[2 * p + 1])));
+        for (int r = 0; r < RI1; ++r) no[r] = -fminf(O_INIT, floorf(cm[r]));
     }
     float omax_w = O_INIT;            // warp-uniform upper bound of this warp's offsets (culling test)
     if (CULL) {
         float om = -3.0e38f;
 #pragma unroll
-        for (int p = 0; p < NPAIR1; ++p) { const float2 nv = unpack2(no[p]); om = fmaxf(om, fmaxf(-nv.x, -nv.y)); }
+        for (int r = 0; r < RI1; ++r) om = fmaxf(om, -no[r]);
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) om = fmaxf(om, __shfl_xor_sync(0xffffffffu, om, o));
         omax_w = om;
@@ -604,7 +586,7 @@ pass1_kernel(const float4* __restrict__ ipts, int ni, const float4* __restrict__
     for (int it = 0; it < nst; ++it) {
         const int s = it % NSTAGE;
         mbar_wait(&full[s], (uint32_t)((it / NSTAGE) & 1));
-        const ulonglong2* sp = reinterpret_cast<const ulonglong2*>(smraw + s * P1_STAGE_BYTES);
+        const float4* sp = reinterpret_cast<const float4*>(smraw + s * P1_STAGE_BYTES);
         bool skip = false;
         if (CULL) {      // every pair of (this warp, this stage) has t' = u - o >= CULL_GAP: exactly zero terms
             const float4 blo = sbox[2 * (st0 + it)], bhi = sbox[2 * (st0 + it) + 1];
@@ -616,52 +598,36 @@ pass1_kernel(const float4* __restrict__ ipts, int ni, const float4* __restrict__
                 const int sb = (st0 + it) * (P1_STAGE / SUB) + sc;
                 if (box_gap2(mybox, ssub[2 * sb], ssub[2 * sb + 1]) - omax_w >= CULL_GAP) continue;
             }
-            const ulonglong2* q = sp + sc * (2 * SUB);
-            u64 Sc[NPAIR1], Uc[NPAIR1];          // Sc = sum e,  Uc = sum e * t'  with t' = u - o, e = 2^-t'
+            const float4* q = sp + sc * SUB;
+            float Sc[RI1], Uc[RI1];          // Sc = sum e,  Uc = sum e * t'  with t' = u - o, e = 2^-t'
 #pragma unroll
-            for (int p = 0; p < NPAIR1; ++p) { Sc[p] = 0ull; Uc[p] = 0ull; }
+            for (int r = 0; r < RI1; ++r) { Sc[r] = 0.0f; Uc[r] = 0.0f; }
             pass1_sum<WGT>(q, ax, ay, az, no, Sc, Uc);
             bool bad = false;
 #pragma unroll
-            for (int p = 0; p < NPAIR1; ++p) {
-                const float2 v = unpack2(Sc[p]);
-                bad |= !(v.x < TWO100) | !(v.y < TWO100);
-            }
+            for (int r = 0; r < RI1; ++r) bad |= !(Sc[r] < TWO100);
             if (__any_sync(0xffffffffu, bad)) {
                 float cm[RI1];
 #pragma unroll
                 for (int r = 0; r < RI1; ++r) cm[r] = 3.0e38f;
 #pragma unroll UNROLL1
                 for (int jj = 0; jj < SUB; ++jj) {
-                    const ulonglong2 bxy = q[2 * jj];
-                    const u64 bz = q[2 * jj + 1].x;
-                    u64 la = 0ull;
-                    if (WGT) la = q[2 * jj + 1].y;
+                    const float4 b = q[jj];
 #pragma unroll
-                    for (int p = 0; p < NPAIR1; ++p) {
-                        const u64 dx = fsub2(ax[p], bxy.x), dy = fsub2(ay[p], bxy.y), dz = fsub2(az[p], bz);
-                        u64 uu = ffma2(dz, dz, ffma2(dy, dy, fmul2(dx, dx)));
-                        if (WGT) uu = fadd2(uu, la);
-                        const float2 u = unpack2(uu);
-                        cm[2 * p] = fminf(cm[2 * p], u.x);
-                        cm[2 * p + 1] = fminf(cm[2 * p + 1], u.y);
-                    }
+                    for (int r = 0; r < RI1; ++r) cm[r] = fminf(cm[r], pass1_u<WGT>(ax[r], ay[r], az[r], b));
                 }
 #pragma unroll
-                for (int p = 0; p < NPAIR1; ++p) {
-                    const float2 nv = unpack2(no[p]);
-                    const float o0 = -nv.x, o1 = -nv.y;
-                    const float on0 = fminf(o0, floorf(cm[2 * p])), on1 = fminf(o1, floorf(cm[2 * p + 1]));
-                    const int sh0 = (int)fmaxf(on0 - o0, -4000.0f), sh1 = (int)fmaxf(on1 - o1, -4000.0f);
-                    S[2 * p] = ldexp(S[2 * p], sh0); SU[2 * p] = ldexp(SU[2 * p], sh0);
-                    S[2 * p + 1] = ldexp(S[2 * p + 1], sh1); SU[2 * p + 1] = ldexp(SU[2 * p + 1], sh1);
-                    no[p] = pack2(-on0, -on1);
-                    Sc[p] = 0ull; Uc[p] = 0ull;
+                for (int r = 0; r < RI1; ++r) {
+                    const float o = -no[r], on = fminf(o, floorf(cm[r]));
+                    const int sh = (int)fmaxf(on - o, -4000.0f);
+                    S[r] = ldexp(S[r], sh); SU[r] = ldexp(SU[r], sh);
+                    no[r] = -on;
+                    Sc[r] = 0.0f; Uc[r] = 0.0f;
                 }
                 if (CULL) {      // the offsets just dropped: tighten the warp's bound for the culling test
                     float om = -3.0e38f;
 #pragma unroll
-                    for (int p = 0; p < NPAIR1; ++p) { const float2 nv = unpack2(no[p]); om = fmaxf(om, fmaxf(-nv.x, -nv.y)); }
+                    for (int r = 0; r < RI1; ++r) om = fmaxf(om, -no[r]);
 #pragma unroll
                     for (int o = 16; o > 0; o >>= 1) om = fmaxf(om, __shfl_xor_sync(0xffffffffu, om, o));
                     omax_w = om;
@@ -669,12 +635,9 @@ pass1_kernel(const float4* __restrict__ ipts, int ni, const float4* __restrict__
                 pass1_sum<WGT>(q, ax, ay, az, no, Sc, Uc);
             }
 #pragma unroll
-            for (int p = 0; p < NPAIR1; ++p) {
-                const float2 sv = unpack2(Sc[p]), uv = unpack2(Uc[p]), nv = unpack2(no[p]);
-                S[2 * p] += (double)sv.x;
-                S[2 * p + 1] += (double)sv.y;
-                SU[2 * p] += (double)uv.x - (double)nv.x * (double)sv.x;         // sum e*u = sum e*t' + o * sum e
-                SU[2 * p + 1] += (double)uv.y - (double)nv.y * (double)sv.y;
+            for (int r = 0; r < RI1; ++r) {
+                S[r] += (double)Sc[r];
+                SU[r] += (double)Uc[r] - (double)no[r] * (double)Sc[r];         // sum e*u = sum e*t' + o * sum e
             }
         }
         __syncthreads();
@@ -684,16 +647,12 @@ pass1_kernel(const float4* __restrict__ ipts, int ni, const float4* __restrict__
         }
     }
 #pragma unroll
-    for (int p = 0; p < NPAIR1; ++p) {
-        const float2 nv = unpack2(no[p]);
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int n = itile * ITILE1 + (tid >> 5) * (32 * RI1) + (2 * p + h) * 32 + (tid & 31);
-            if (n < ni) {
-                P1Part out;
-                out.S = S[2 * p + h]; out.SU = SU[2 * p + h]; out.o = h ? -nv.y : -nv.x; out.pad = 0.0f;
-                part[(size_t)split * ni + n] = out;
-            }
+    for (int r = 0; r < RI1; ++r) {
+        const int n = itile * ITILE1 + (tid >> 5) * (32 * RI1) + r * 32 + (tid & 31);
+        if (n < ni) {
+            P1Part out;
+            out.S = S[r]; out.SU = SU[r]; out.o = -no[r]; out.pad = 0.0f;
+            part[(size_t)split * ni + n] = out;
         }
     }
 }
@@ -708,7 +667,7 @@ pass1_kernel(const float4* __restrict__ ipts, int ni, const float4* __restrict__
 //   L      = log2(den) = log2(2^log2S + c)          c = (2 pi s2)^(D/2) w/(1-w) M/N  (cpd.py:78-79)
 //   pt1    = 2^(log2S - L)                          (cpd.py:85; == 1 when w == 0)
 //   rn     = 2^(-omin) / den = 2^-(L + omin)        P_mn = 2^(omin - u_mn) * rn in pass 2
-//   record = {bx,bx,by,by},{bz,bz,-omin,-omin},{rn,rn,0,0}   (48 B, duplicated for the pair inner loop)
+//   record = {bx,by,bz,-omin},{rn,0,0,0}   (32 B: 16-byte aligned for the bulk copy)
 //            dead / padding: -omin = +inf (so 2^-(u - omin) == 0), rn = 0
 // and the target-side moments: Srr = sum_n SU_n rn_n (= sum_mn P_mn u_mn), Npt = sum pt1.
 // ---------------------------------------------------------------------------------------------
@@ -768,20 +727,18 @@ finalize1_kernel(const DevState* __restrict__ st, const double* __restrict__ sig
             v[0] = SU * (double)rnf;       // the same (rounded) rn that pass 2 multiplies by
         }
         v[1] = p1n;
-        tgtQ[3 * (size_t)i] = make_float4(b.x, b.x, b.y, b.y);
-        tgtQ[3 * (size_t)i + 1] = make_float4(b.z, b.z, no, no);
-        tgtQ[3 * (size_t)i + 2] = make_float4(rnf, rnf, 0.f, 0.f);
+        tgtQ[2 * (size_t)i] = make_float4(b.x, b.y, b.z, no);
+        tgtQ[2 * (size_t)i + 1] = make_float4(rnf, 0.f, 0.f, 0.f);
     } else if (i < npad) {
-        tgtQ[3 * (size_t)i] = make_float4(0.f, 0.f, 0.f, 0.f);
-        tgtQ[3 * (size_t)i + 1] = make_float4(0.f, 0.f, INFINITY, INFINITY);
-        tgtQ[3 * (size_t)i + 2] = make_float4(0.f, 0.f, 0.f, 0.f);
+        tgtQ[2 * (size_t)i] = make_float4(0.f, 0.f, 0.f, INFINITY);
+        tgtQ[2 * (size_t)i + 1] = make_float4(0.f, 0.f, 0.f, 0.f);
     }
     block_reduce_store<RM_TGT>(v, mom_part + (size_t)blockIdx.x * RM_TGT);
 }
 
 // ---------------------------------------------------------------------------------------------
 // pass 2: per source m and split of the targets:  p1_m = sum_n P_mn,  sd_m = sum_n P_mn (a_m - b_n)
-// with P_mn = 2^(o_n - u_mn) * rn_n.  Per two pairs: 11 packed FP32 instructions + 2 MUFU.
+// with P_mn = 2^(o_n - u_mn) * rn_n.  Per pair: 11 FP32 instructions + 1 MUFU.EX2.
 // ---------------------------------------------------------------------------------------------
 template <bool CULL, bool WGT>
 __global__ void __launch_bounds__(THREADS, CPD_MINB2)
@@ -807,25 +764,23 @@ pass2_kernel(const float4* __restrict__ ipts, int ni, const float4* __restrict__
             tma_load_1d(smraw + s * P2_STAGE_BYTES, jbytes + (size_t)(st0 + s) * P2_STAGE_BYTES, P2_STAGE_BYTES, &full[s]);
         }
     }
-    u64 ax[NPAIR2], ay[NPAIR2], az[NPAIR2], al[NPAIR2];      // al = (la, la') of the two sources: WGT only
+    float ax[RI2], ay[RI2], az[RI2], al[RI2];      // al = la of the source: WGT only
     double A1[RI2], AX[RI2], AY[RI2], AZ[RI2];
 #pragma unroll
-    for (int p = 0; p < NPAIR2; ++p) {
-        int m0 = itile * ITILE2 + (tid >> 5) * (32 * RI2) + (2 * p) * 32 + (tid & 31), m1 = m0 + 32;
-        m0 = m0 < ni ? m0 : ni - 1;
-        m1 = m1 < ni ? m1 : ni - 1;
-        const float4 p0 = ipts[m0], p1 = ipts[m1];
-        ax[p] = pack2(p0.x, p1.x); ay[p] = pack2(p0.y, p1.y); az[p] = pack2(p0.z, p1.z);
-        if (WGT) al[p] = pack2(p0.w, p1.w);
+    for (int r = 0; r < RI2; ++r) {
+        int m = itile * ITILE2 + (tid >> 5) * (32 * RI2) + r * 32 + (tid & 31);
+        m = m < ni ? m : ni - 1;
+        const float4 p = ipts[m];
+        ax[r] = p.x; ay[r] = p.y; az[r] = p.z; al[r] = p.w;
     }
     float* const mybox = wbox[tid >> 5];
-    if (CULL) warp_bbox<NPAIR2>(ax, ay, az, mybox);
+    if (CULL) warp_bbox<RI2>(ax, ay, az, mybox);
 #pragma unroll
     for (int r = 0; r < RI2; ++r) { A1[r] = 0.0; AX[r] = 0.0; AY[r] = 0.0; AZ[r] = 0.0; }
     for (int it = 0; it < nst; ++it) {
         const int s = it % NSTAGE;
         mbar_wait(&full[s], (uint32_t)((it / NSTAGE) & 1));
-        const ulonglong2* sp = reinterpret_cast<const ulonglong2*>(smraw + s * P2_STAGE_BYTES);
+        const float4* sp = reinterpret_cast<const float4*>(smraw + s * P2_STAGE_BYTES);
         bool skip = false;
         if (CULL) {
             const float4 blo = tbox[2 * (st0 + it)], bhi = tbox[2 * (st0 + it) + 1];
@@ -837,67 +792,60 @@ pass2_kernel(const float4* __restrict__ ipts, int ni, const float4* __restrict__
                 const int sb = (st0 + it) * (P2_STAGE / SUB) + sc;
                 if (box_gap2(mybox, tsub[2 * sb], tsub[2 * sb + 1]) - omax_sub[sb] >= CULL_GAP) continue;
             }
-            const ulonglong2* q = sp + sc * (3 * SUB);
-            u64 s1[NPAIR2], sx[NPAIR2], sy[NPAIR2], sz[NPAIR2];
+            const float4* q = sp + sc * (2 * SUB);
+            float s1[RI2], sx[RI2], sy[RI2], sz[RI2];
 #pragma unroll
-            for (int p = 0; p < NPAIR2; ++p) { s1[p] = 0ull; sx[p] = 0ull; sy[p] = 0ull; sz[p] = 0ull; }
+            for (int r = 0; r < RI2; ++r) { s1[r] = 0.0f; sx[r] = 0.0f; sy[r] = 0.0f; sz[r] = 0.0f; }
             if (GRP > 0) {
-#pragma unroll 1
+                // two groups per trip: the second group's FP32 work overlaps the first one's EX2 tail (measured on the H100: 4 %
+                // less pass-2 time); not in the culled weighted instantiation, which would then spill at the 128-register cap
+#pragma unroll (CULL && WGT) ? 1 : 2
                 for (int g0 = 0; g0 < SUB; g0 += (GRP > 0 ? GRP : SUB)) {
-                    u64 g1[NPAIR2], gx[NPAIR2], gy[NPAIR2], gz[NPAIR2];
+                    float g1[RI2], gx[RI2], gy[RI2], gz[RI2];
 #pragma unroll
                     for (int jj = 0; jj < (GRP > 0 ? GRP : 1); ++jj) {
-                        const ulonglong2 bxy = q[3 * (g0 + jj)];
-                        const ulonglong2 bzo = q[3 * (g0 + jj) + 1];
-                        const u64 rn = q[3 * (g0 + jj) + 2].x;
+                        const float4 b = q[2 * (g0 + jj)];
+                        const float rn = q[2 * (g0 + jj) + 1].x;
 #pragma unroll
-                        for (int p = 0; p < NPAIR2; ++p) {
-                            const u64 dx = fsub2(ax[p], bxy.x), dy = fsub2(ay[p], bxy.y), dz = fsub2(az[p], bzo.x);
-                            u64 t = ffma2(dx, dx, bzo.y);         // t' = u - o_n: the same FMA chain and offset as pass 1
-                            t = ffma2(dy, dy, t);
-                            t = ffma2(dz, dz, t);
-                            if (WGT) t = fadd2(t, al[p]);
-                            const float2 tt = unpack2(t);
-                            const u64 pr = fmul2(pack2(ex2(-tt.x), ex2(-tt.y)), rn);
-                            g1[p] = jj == 0 ? pr : fadd2(g1[p], pr);
-                            gx[p] = jj == 0 ? fmul2(pr, dx) : ffma2(pr, dx, gx[p]);
-                            gy[p] = jj == 0 ? fmul2(pr, dy) : ffma2(pr, dy, gy[p]);
-                            gz[p] = jj == 0 ? fmul2(pr, dz) : ffma2(pr, dz, gz[p]);
+                        for (int r = 0; r < RI2; ++r) {
+                            const float dx = __fsub_rn(ax[r], b.x), dy = __fsub_rn(ay[r], b.y), dz = __fsub_rn(az[r], b.z);
+                            // t' = u - o_n: the same FMA chain and offset as pass 1
+                            float t = __fmaf_rn(dz, dz, __fmaf_rn(dy, dy, __fmaf_rn(dx, dx, b.w)));
+                            if (WGT) t = __fadd_rn(t, al[r]);
+                            const float pr = __fmul_rn(ex2(-t), rn);
+                            g1[r] = jj == 0 ? pr : __fadd_rn(g1[r], pr);
+                            gx[r] = jj == 0 ? __fmul_rn(pr, dx) : __fmaf_rn(pr, dx, gx[r]);
+                            gy[r] = jj == 0 ? __fmul_rn(pr, dy) : __fmaf_rn(pr, dy, gy[r]);
+                            gz[r] = jj == 0 ? __fmul_rn(pr, dz) : __fmaf_rn(pr, dz, gz[r]);
                         }
                     }
 #pragma unroll
-                    for (int p = 0; p < NPAIR2; ++p) {
-                        s1[p] = fadd2(s1[p], g1[p]); sx[p] = fadd2(sx[p], gx[p]);
-                        sy[p] = fadd2(sy[p], gy[p]); sz[p] = fadd2(sz[p], gz[p]);
+                    for (int r = 0; r < RI2; ++r) {
+                        s1[r] = __fadd_rn(s1[r], g1[r]); sx[r] = __fadd_rn(sx[r], gx[r]);
+                        sy[r] = __fadd_rn(sy[r], gy[r]); sz[r] = __fadd_rn(sz[r], gz[r]);
                     }
                 }
             } else {
 #pragma unroll UNROLL2
                 for (int jj = 0; jj < SUB; ++jj) {
-                    const ulonglong2 bxy = q[3 * jj];
-                    const ulonglong2 bzo = q[3 * jj + 1];
-                    const u64 rn = q[3 * jj + 2].x;
+                    const float4 b = q[2 * jj];
+                    const float rn = q[2 * jj + 1].x;
 #pragma unroll
-                    for (int p = 0; p < NPAIR2; ++p) {
-                        const u64 dx = fsub2(ax[p], bxy.x), dy = fsub2(ay[p], bxy.y), dz = fsub2(az[p], bzo.x);
-                        u64 t = ffma2(dx, dx, bzo.y);
-                        t = ffma2(dy, dy, t);
-                        t = ffma2(dz, dz, t);
-                        if (WGT) t = fadd2(t, al[p]);
-                        const float2 tt = unpack2(t);
-                        const u64 pr = fmul2(pack2(ex2(-tt.x), ex2(-tt.y)), rn);
-                        s1[p] = fadd2(s1[p], pr);
-                        sx[p] = ffma2(pr, dx, sx[p]);
-                        sy[p] = ffma2(pr, dy, sy[p]);
-                        sz[p] = ffma2(pr, dz, sz[p]);
+                    for (int r = 0; r < RI2; ++r) {
+                        const float dx = __fsub_rn(ax[r], b.x), dy = __fsub_rn(ay[r], b.y), dz = __fsub_rn(az[r], b.z);
+                        float t = __fmaf_rn(dz, dz, __fmaf_rn(dy, dy, __fmaf_rn(dx, dx, b.w)));
+                        if (WGT) t = __fadd_rn(t, al[r]);
+                        const float pr = __fmul_rn(ex2(-t), rn);
+                        s1[r] = __fadd_rn(s1[r], pr);
+                        sx[r] = __fmaf_rn(pr, dx, sx[r]);
+                        sy[r] = __fmaf_rn(pr, dy, sy[r]);
+                        sz[r] = __fmaf_rn(pr, dz, sz[r]);
                     }
                 }
             }
 #pragma unroll
-            for (int p = 0; p < NPAIR2; ++p) {
-                const float2 v1 = unpack2(s1[p]), vx = unpack2(sx[p]), vy = unpack2(sy[p]), vz = unpack2(sz[p]);
-                A1[2 * p] += (double)v1.x; AX[2 * p] += (double)vx.x; AY[2 * p] += (double)vy.x; AZ[2 * p] += (double)vz.x;
-                A1[2 * p + 1] += (double)v1.y; AX[2 * p + 1] += (double)vx.y; AY[2 * p + 1] += (double)vy.y; AZ[2 * p + 1] += (double)vz.y;
+            for (int r = 0; r < RI2; ++r) {
+                A1[r] += (double)s1[r]; AX[r] += (double)sx[r]; AY[r] += (double)sy[r]; AZ[r] += (double)sz[r];
             }
         }
         __syncthreads();
