@@ -261,6 +261,39 @@ int cpd_ocsvm_fit(int device, const double* x, int64_t n, int dim, double nu, do
 int cpd_squared_kernel_sum(int device, const double* x, int64_t nx, const double* y, int64_t ny,
                            int dim, double* out);
 
+/* FilterReg (probreg/filterreg.py, gaussian_filtering.py; csrc/lattice.cuh), without a handle.  The permutohedral lattice is the
+ * reference's x86-64 build (third_party/permutohedral, SSE path) reproduced bit for bit: the same vertex set and lattice size,
+ * including the vertices of the zero padding lanes of its 4-point blocks, and the same float32 splat, blur and slice, with
+ * compute()'s dispatch (seqCompute for 1-2 value channels, sseCompute for 3 or more).
+ * cpd_lattice_filter: Permutohedral(feature, with_blur) over n points (n x d float32, row-major, |feature| < 1e8), then
+ *   filter(values) of vs = 1..8 channels (n x vs float32) into out (n x vs).  values == NULL: only *lattice_size.
+ * cpd_filterreg_estep: FilterReg.expectation_step (filterreg.py:78-108) on t_source (m x d) and target (n x d): the features
+ *   float32(x / sqrt(sigma2)), the blurred lattice, rebuilt without blur when its size exceeds n * alpha (*with_blur tells which),
+ *   and m0 (m), m1 (m x d), m2 (m, update_sigma2 only; |y|^2 in FP64 rounded once) and nx (m x d, target_normals != NULL only)
+ *   read at the sources.  stage_ms (NULL or 6 floats): ms of [0] elevation [1] sort [2] vertex numbering and blur neighbours
+ *   [3] splat [4] blur [5] slice, of the last lattice built.                                                                  */
+int cpd_lattice_filter(int device, const float* feature, int64_t n, int d, const float* values, int vs, int with_blur, float* out,
+                       int64_t* lattice_size);
+int cpd_filterreg_estep(int device, const double* t_source, int64_t m, const double* target, int64_t n, int d,
+                        const double* target_normals, double sigma2, int update_sigma2, double alpha, float* m0, float* m1, float* m2,
+                        float* nx, int* with_blur, float* stage_ms);
+/* The FilterReg loop (filterreg.py:120-147) with the clouds resident on the device.  cpd_filterreg_begin uploads source (m x d),
+ * target (n x d) and target_normals (n x d, NULL for pt2pt) once.  cpd_filterreg_step(h, rot (d x d row-major), t, sigma2, w, moments)
+ * moves the source in FP64 (x' = ((R00 x + R01 y) + R02 z) + t0, no FMA), runs the E-step of cpd_filterreg_estep on it and
+ * reduces the M-step's sums (filterreg.py:163-196) over the sources with m0 != 0 in FP64, fixed order, into 49 doubles:
+ *   [0] survivors  [1] S wt  [2..4] S wt x  [5..7] S wt y  [8] S wt^2  [9] S wt |x - y|  [10] S (m0 |x|^2 - 2 x.m1 + m2) / (m0 + c)
+ *   [11] S m0 / (m0 + c)  [12..20] S wt^2 (x - mc)(y - tc)^T (3 x 3, mc, tc the wt-weighted centres)
+ *   [21..41] S wt J J^T (upper triangle, row by row)  [42..47] S wt r J  [48] S wt^2 r^2   (point to plane, 3-D with normals)
+ * with y = m1 / m0, c = w / (1 - w) n / m (2 pi sigma2)^(d/2), wt = sqrt(m0 / (m0 + c) / sigma2), n = nx / m0, r = n.(y - x),
+ * J = [x cross n, n]; coordinates past d are 0.  Only these doubles cross per step.  cpd_filterreg_get reads the last E-step's
+ * m0, m1, m2, nx (NULL: skipped), the blur decision, the device bytes the handle holds and the last step's stage times.      */
+typedef struct cpd_fr cpd_fr;
+int cpd_filterreg_begin(cpd_fr** out, int device, const double* source, int64_t m, const double* target, int64_t n, int d,
+                        const double* target_normals, int update_sigma2, double alpha);
+int cpd_filterreg_step(cpd_fr* h, const double* rot, const double* t, double sigma2, double w, double* moments);
+int cpd_filterreg_get(cpd_fr* h, float* m0, float* m1, float* m2, float* nx, int* with_blur, int64_t* device_bytes, float* stage_ms);
+void cpd_filterreg_end(cpd_fr* h);
+
 /* -- multi-GPU: one process per GPU, targets sharded, sources replicated -------------------
  * cpd_comm_unique_id fills 128 bytes (an ncclUniqueId) on one rank; after it has been
  * distributed (any side channel), every rank calls cpd_comm_create ONCE -- a collective -- and

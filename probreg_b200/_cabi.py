@@ -80,6 +80,16 @@ _PROTOS = {
     "cpd_tps_kernel": (ctypes.c_int, [ctypes.c_int, _c_dp, ctypes.c_int64, _c_dp, ctypes.c_int64, ctypes.c_int, _c_fp]),
     "cpd_ocsvm_fit": (ctypes.c_int, [ctypes.c_int, _c_dp, ctypes.c_int64, ctypes.c_int, ctypes.c_double, ctypes.c_double, ctypes.c_double,
                                      ctypes.c_int64, _c_dp, _c_dp, ctypes.POINTER(ctypes.c_int64)]),
+    "cpd_lattice_filter": (ctypes.c_int, [ctypes.c_int, _c_fp, ctypes.c_int64, ctypes.c_int, _c_fp, ctypes.c_int, ctypes.c_int, _c_fp,
+                                          ctypes.POINTER(ctypes.c_int64)]),
+    "cpd_filterreg_estep": (ctypes.c_int, [ctypes.c_int, _c_dp, ctypes.c_int64, _c_dp, ctypes.c_int64, ctypes.c_int, _c_dp, ctypes.c_double,
+                                           ctypes.c_int, ctypes.c_double, _c_fp, _c_fp, _c_fp, _c_fp, ctypes.POINTER(ctypes.c_int), _c_fp]),
+    "cpd_filterreg_begin": (ctypes.c_int, [ctypes.POINTER(ctypes.c_void_p), ctypes.c_int, _c_dp, ctypes.c_int64, _c_dp, ctypes.c_int64,
+                                           ctypes.c_int, _c_dp, ctypes.c_int, ctypes.c_double]),
+    "cpd_filterreg_step": (ctypes.c_int, [ctypes.c_void_p, _c_dp, _c_dp, ctypes.c_double, ctypes.c_double, _c_dp]),
+    "cpd_filterreg_get": (ctypes.c_int, [ctypes.c_void_p, _c_fp, _c_fp, _c_fp, _c_fp, ctypes.POINTER(ctypes.c_int),
+                                         ctypes.POINTER(ctypes.c_int64), _c_fp]),
+    "cpd_filterreg_end": (None, [ctypes.c_void_p]),
     "cpd_squared_kernel_sum": (ctypes.c_int, [ctypes.c_int, _c_dp, ctypes.c_int64, _c_dp, ctypes.c_int64, ctypes.c_int, _c_dp]),
     "cpd_comm_unique_id": (ctypes.c_int, [ctypes.c_char_p]),
     "cpd_comm_create": (ctypes.c_int, [ctypes.POINTER(ctypes.c_void_p), ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_char_p]),
@@ -565,6 +575,105 @@ def ocsvm_fit(x, nu, gamma, tol=1e-3, max_iter=None, device=0):
     check(lib().cpd_ocsvm_fit(device, dptr(xa), n, xa.shape[1], float(nu), float(gamma), float(tol), max_iter, dptr(alpha),
                               ctypes.byref(rho), ctypes.byref(it)))
     return alpha, rho.value, it.value
+
+
+def fptr(a):
+    return None if a is None else a.ctypes.data_as(_c_fp)
+
+
+def lattice_filter(feature, values=None, with_blur=True, device=0):
+    """(filtered values (n x vs float32) or None, lattice size) of the reference's permutohedral lattice (cpd_lattice_filter):
+    Permutohedral(feature, with_blur).filter(values) with feature and values rounded to float32 as pybind11 rounds them."""
+    f = np.ascontiguousarray(feature, dtype=np.float32)
+    if f.ndim != 2:
+        raise ValueError("feature must be (n x d), got shape %s" % (f.shape,))
+    n, d = f.shape
+    size = ctypes.c_int64()
+    if values is None:
+        check(lib().cpd_lattice_filter(device, fptr(f), n, d, None, 0, int(bool(with_blur)), None, ctypes.byref(size)))
+        return None, size.value
+    v = np.ascontiguousarray(values, dtype=np.float32)
+    if v.ndim == 1:
+        v = v[:, None]
+    if v.ndim != 2 or v.shape[0] != n:
+        raise ValueError("values must have one row per feature point: %s for %d points" % (v.shape, n))
+    out = np.empty_like(v)
+    check(lib().cpd_lattice_filter(device, fptr(f), n, d, fptr(v), v.shape[1], int(bool(with_blur)), fptr(out), ctypes.byref(size)))
+    return out, size.value
+
+
+def filterreg_estep(t_source, target, sigma2, update_sigma2, target_normals=None, alpha=0.015, device=0, stage_ms=None):
+    """(m0, m1, m2 or None, nx or None, with_blur) of FilterReg.expectation_step on the device (cpd_filterreg_estep), float32."""
+    s, t = as_cloud(t_source), as_cloud(target)
+    m, d = s.shape
+    n = t.shape[0]
+    if t.shape[1] != d:
+        raise ValueError("source and target must have the same dimension: %d and %d" % (d, t.shape[1]))
+    nrm = None if target_normals is None else as_cloud(target_normals, d)
+    if nrm is not None and nrm.shape[0] != n:
+        raise ValueError("target_normals must have one row per target point: %d for %d" % (nrm.shape[0], n))
+    m0, m1 = np.empty(m, np.float32), np.empty((m, d), np.float32)
+    m2 = np.empty(m, np.float32) if update_sigma2 else None
+    nx = np.empty((m, d), np.float32) if nrm is not None else None
+    blur = ctypes.c_int()
+    check(lib().cpd_filterreg_estep(device, dptr(s), m, dptr(t), n, d, dptr(nrm) if nrm is not None else None, float(sigma2),
+                                    int(bool(update_sigma2)), float(alpha), fptr(m0), fptr(m1), fptr(m2), fptr(nx), ctypes.byref(blur),
+                                    fptr(stage_ms)))
+    return m0, m1, m2, nx, bool(blur.value)
+
+
+class FilterRegLoop(object):
+    """The FilterReg loop's device state (cpd_filterreg_begin / step / get / end): the clouds uploaded once; step() moves the
+    source, runs the E-step and returns the 49 FP64 M-step sums of include/cpd_b200.h."""
+    N_MOMENTS = 49
+
+    def __init__(self, source, target, target_normals=None, update_sigma2=False, alpha=0.015, device=0):
+        s, t = as_cloud(source), as_cloud(target)
+        if t.shape[1] != s.shape[1]:
+            raise ValueError("source and target must have the same dimension: %d and %d" % (s.shape[1], t.shape[1]))
+        nrm = None if target_normals is None else as_cloud(target_normals, s.shape[1])
+        if nrm is not None and nrm.shape[0] != t.shape[0]:
+            raise ValueError("target_normals must have one row per target point: %d for %d" % (nrm.shape[0], t.shape[0]))
+        self.m, self.d = s.shape
+        self.update_sigma2, self.has_normals = bool(update_sigma2), nrm is not None
+        self._lib = lib()
+        h = ctypes.c_void_p()
+        check(self._lib.cpd_filterreg_begin(ctypes.byref(h), device, dptr(s), self.m, dptr(t), t.shape[0], self.d, dptr(nrm),
+                                            int(self.update_sigma2), float(alpha)))
+        self._h = h
+
+    def step(self, rot, t, sigma2, w):
+        mom = np.empty(self.N_MOMENTS)
+        r = np.ascontiguousarray(rot, np.float64)
+        tt = np.ascontiguousarray(t, np.float64)
+        check(self._lib.cpd_filterreg_step(self._h, dptr(r), dptr(tt), float(sigma2), float(w), dptr(mom)))
+        return mom
+
+    def last_estep(self):
+        """(m0, m1, m2 or None, nx or None, with_blur) of the last step's E-step."""
+        m, d = self.m, self.d
+        m0, m1 = np.empty(m, np.float32), np.empty((m, d), np.float32)
+        m2 = np.empty(m, np.float32) if self.update_sigma2 else None
+        nx = np.empty((m, d), np.float32) if self.has_normals else None
+        blur = ctypes.c_int()
+        check(self._lib.cpd_filterreg_get(self._h, fptr(m0), fptr(m1), fptr(m2), fptr(nx), ctypes.byref(blur), None, None))
+        return m0, m1, m2, nx, bool(blur.value)
+
+    def device_bytes(self):
+        b = ctypes.c_int64()
+        check(self._lib.cpd_filterreg_get(self._h, None, None, None, None, None, ctypes.byref(b), None))
+        return b.value
+
+    def stage_ms(self):
+        ms = np.zeros(6, np.float32)
+        check(self._lib.cpd_filterreg_get(self._h, None, None, None, None, None, None, fptr(ms)))
+        return ms
+
+    def __del__(self):
+        h = getattr(self, "_h", None)
+        if h is not None and h.value:
+            self._lib.cpd_filterreg_end(h)
+            self._h = None
 
 
 def comm_create(device, world_size, rank, uid):

@@ -9,6 +9,7 @@
 #include "gmmtree.cuh"
 #include "l2dist.cuh"
 #include "ocsvm.cuh"
+#include "lattice.cuh"
 
 #include <cub/device/device_radix_sort.cuh>
 #ifdef CPD_HOST_EMU
@@ -1121,5 +1122,6 @@ extern "C" int cpd_mstep(cpd_ctx* h, int tf_kind, int update_scale, const double
 #include "host_stateless.inl"    // cpd_rbf_kernel, cpd_imq_kernel, cpd_gauss_transform, cpd_squared_kernel_sum
 #include "host_l2dist.inl"       // cpd_gmm_fit, cpd_l2_dist, cpd_tps_kernel (GMMReg)
 #include "host_ocsvm.inl"        // cpd_ocsvm_fit (the one-class SVM of SVR)
+#include "host_filterreg.inl"    // cpd_lattice_filter, cpd_filterreg_estep (the permutohedral lattice of FilterReg)
 #include "host_multi.inl"        // cpd_comm_*, cpd_p2p_*
 #include "host_measure.inl"      // cpd_timer_*, cpd_event_*, cpd_stage_times, cpd_flush_l2, cpd_microbench
