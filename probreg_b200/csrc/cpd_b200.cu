@@ -25,6 +25,8 @@
 #include <string.h>
 
 #include <algorithm>
+#include <memory>
+#include <type_traits>
 #include <vector>
 
 using namespace cpd;
@@ -155,104 +157,178 @@ constexpr int CUDA_R_64F_ = 1, CUBLAS_OP_T_ = 1;
     } while (0)
 
 // ---------------------------------------------------------------------------------------------
+// owners of the handle's resources
+// ---------------------------------------------------------------------------------------------
+#define TRY(x) do { int r__ = (x); if (r__ != CPD_OK) return r__; } while (0)
+namespace {
+// device memory of `n` elements, freed by the destructor
+template <typename T>
+struct DevBuf {
+    T* p = nullptr;
+    size_t n = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    DevBuf(DevBuf&& o) noexcept : p(o.p), n(o.n) { o.p = nullptr; o.n = 0; }
+    DevBuf& operator=(DevBuf&& o) noexcept { std::swap(p, o.p); std::swap(n, o.n); return *this; }
+    ~DevBuf() { reset(); }
+    void reset() {
+        if (p) cudaFree(p);
+        p = nullptr;
+        n = 0;
+    }
+    // exactly `count` elements (at least one is allocated); the old block is freed first and its contents are not kept
+    int alloc(size_t count) {
+        reset();
+        cudaError_t e = cudaMalloc((void**)&p, std::max<size_t>(count, 1) * sizeof(T));
+        if (e != cudaSuccess) {
+            p = nullptr;
+            return fail(CPD_ERR_CUDA, "cudaMalloc(%zu bytes) failed: %s", count * sizeof(T), cudaGetErrorString(e));
+        }
+        n = count;
+        return CPD_OK;
+    }
+    // grow-only: reallocates (as alloc) only when `count` exceeds what is held
+    int reserve(size_t count) { return count > n ? alloc(count) : CPD_OK; }
+    size_t bytes() const { return p ? std::max<size_t>(n, 1) * sizeof(T) : 0; }
+};
+// pinned host memory of `count` elements, freed by the destructor
+template <typename T>
+struct PinBuf {
+    T* p = nullptr;
+    PinBuf() = default;
+    PinBuf(const PinBuf&) = delete;
+    PinBuf& operator=(const PinBuf&) = delete;
+    ~PinBuf() { if (p) cudaFreeHost(p); }
+    int alloc(size_t count) {
+        CU(cudaMallocHost((void**)&p, count * sizeof(T)));
+        return CPD_OK;
+    }
+};
+// an event, destroyed with its owner; converts to cudaEvent_t at use sites
+struct Event {
+    cudaEvent_t e = nullptr;
+    Event() = default;
+    Event(const Event&) = delete;
+    Event& operator=(const Event&) = delete;
+    Event(Event&& o) noexcept : e(o.e) { o.e = nullptr; }
+    ~Event() { if (e) cudaEventDestroy(e); }
+    operator cudaEvent_t() const { return e; }
+};
+#ifndef CPD_HOST_EMU
+struct GraphExecDelete { void operator()(cudaGraphExec_t g) const { cudaGraphExecDestroy(g); } };
+using GraphExec = std::unique_ptr<std::remove_pointer_t<cudaGraphExec_t>, GraphExecDelete>;
+#endif
+// The handle's pinned staging of small host <-> device copies, one field per use: no copy in flight can overwrite another's bytes.
+struct PinStage {
+    DevState state;          // read_params: the device state
+    double sums[8];          // cpd_sigma2_init: target and source sums
+    double es[2];            // cpd_estep, cpd_bcpd_estep: {sigma2, w} into DevState.es_sigma2 / es_w
+    double bc_ssw[3];        // cpd_bcpd_estep: {scale, sigma2, w} into d_bc_es
+    double n_p;              // cpd_last_estep
+    int p2p_err;             // cpd_sync: DevState.err
+    double nr_sigma2_p;      // cpd_nonrigid_mstep: the E-step's sigma2 into DevState.sigma2
+    int nr_info;             // cpd_nonrigid_step / _mstep: getrf's info
+    double bc_sigma2;        // cpd_bcpd_step: the new sigma2
+    int bc_info[2];          // cpd_bcpd_step: getrf's and getrs's info
+    double gmm_lb;           // cpd_gmm_fit: the lower bound of an iteration
+    double gt_q;             // cpd_gmmtree_build: the log-likelihood of an iteration
+    double gt_rt[12];        // cpd_gmmtree_estep: rot (9) and t (3)
+};
+}  // namespace
+
+// ---------------------------------------------------------------------------------------------
 // handle
 // ---------------------------------------------------------------------------------------------
 struct cpd_ctx {
+    // declared first, so destroyed last: the stream the handle created (none when the caller passed one)
+    struct OwnedStream {
+        cudaStream_t s = nullptr;
+        ~OwnedStream() { if (s) cudaStreamDestroy(s); }
+    } owned_stream;
     int device = 0, dim = 3, sm_count = 132, slots1 = 264, slots2 = 264;
     cudaStream_t stream = nullptr;
-    bool own_stream = false;
     long long m = 0, mpad = 0, n = 0, npad = 0, n_global = 0;
-    double *d_yc = nullptr, *d_ts = nullptr, *d_xc = nullptr, *d_raw = nullptr;
-    size_t raw_cap = 0;
-    float4 *d_srcP = nullptr, *d_tgtP = nullptr, *d_tgtQ = nullptr;
-    P1Part* d_part1 = nullptr;
-    double* d_part2 = nullptr;
-    size_t part1_cap = 0, part2_cap = 0;
-    double *d_pt1 = nullptr, *d_p1 = nullptr, *d_pxc = nullptr, *d_px = nullptr;
-    double *d_mom_src = nullptr, *d_mom_tgt = nullptr, *d_mom = nullptr, *d_sums = nullptr;
-    size_t mom_src_cap = 0, mom_tgt_cap = 0, sums_cap = 0;
-    DevState* d_state = nullptr;
+    DevBuf<double> d_yc, d_ts, d_xc, d_raw;
+    DevBuf<float4> d_srcP, d_tgtP, d_tgtQ;
+    DevBuf<P1Part> d_part1;
+    DevBuf<double> d_part2;
+    DevBuf<double> d_pt1, d_p1, d_pxc, d_px;
+    DevBuf<double> d_mom_src, d_mom_tgt, d_mom, d_sums;
+    DevBuf<DevState> d_state;
     DevState h_state;
-    double* h_pin = nullptr;   // 64 pinned doubles for small D2H reads
-    double* d_frame = nullptr;          // [2][8]: what cloud_frame_kernel derives per cloud (sources, targets)
-    double* h_stats = nullptr;          // [2][9] pinned: the clouds' statistics on their way to the host (ensure_stats)
-    cudaEvent_t stats_ev = nullptr, copy_ev = nullptr;
+    PinBuf<PinStage> pin;
+    DevBuf<double> d_frame;             // [2][8]: what cloud_frame_kernel derives per cloud (sources, targets)
+    PinBuf<double> h_stats;             // [2][9] pinned: the clouds' statistics on their way to the host (ensure_stats)
+    Event stats_ev, copy_ev;
     int stats_pending = 0;              // bit 0: sources, bit 1: targets
     long long stats_count[2] = {0, 0};
     bool origin_given = false;
     int it1 = 0, it2 = 0, j1 = 1, j2 = 1, g1 = 1, g2 = 1;   // i-tiles, max partial slots per tile, work items (= grid)
     // exact culling of far blocks (late iterations): stage bounding boxes, per-stage max offset
-    float4 *d_sbox = nullptr, *d_tbox = nullptr, *d_ssub = nullptr, *d_tsub = nullptr;
-    float *d_omax = nullptr, *d_omax_sub = nullptr;
+    DevBuf<float4> d_sbox, d_tbox, d_ssub, d_tsub;
+    DevBuf<float> d_omax, d_omax_sub;
     bool cull_on = true, cull_active = false;
     double extent = 0.0;              // largest bounding-box edge of the target shard (caller units)
-    int4 *d_work1 = nullptr, *d_work2 = nullptr;
-    int *d_slots1 = nullptr, *d_slots2 = nullptr;
+    DevBuf<int4> d_work1, d_work2;
+    DevBuf<int> d_slots1, d_slots2;
     bool have_source = false, have_target = false, have_state = false, prepared = false;
     nccl_comm comm = nullptr;
     int world = 1, rank = 0;
     // Morton ordering (internal permutation; results leave in the caller's order)
-    int *d_perm_src = nullptr, *d_perm_tgt = nullptr, *d_idx_tmp = nullptr;
-    unsigned *d_codes = nullptr, *d_codes_out = nullptr;
-    size_t sort_cap = 0, sort_tmp_cap = 0;
-    void* d_sort_tmp = nullptr;
-    double *d_outN = nullptr, *d_outM = nullptr;      // staging for un-permuted outputs / permuted inputs
+    DevBuf<int> d_perm_src, d_perm_tgt, d_idx_tmp;
+    DevBuf<unsigned> d_codes, d_codes_out;
+    DevBuf<unsigned char> d_sort_tmp;
+    DevBuf<double> d_outN, d_outM;      // staging for un-permuted outputs / permuted inputs
     // non-rigid CPD (dense G)
-    float* d_G = nullptr;
-    double *d_W = nullptr, *d_A = nullptr, *d_B = nullptr, *d_ts2 = nullptr, *d_nrpart = nullptr;
-    int64_t* d_ipiv = nullptr;
-    int* d_info = nullptr;
-    void *d_work = nullptr, *h_work = nullptr, *sol = nullptr, *sol_params = nullptr;
-    size_t work_dev = 0, work_host = 0;
+    DevBuf<float> d_G;
+    DevBuf<double> d_W, d_A, d_B, d_ts2, d_nrpart;
+    DevBuf<int64_t> d_ipiv;
+    DevBuf<int> d_info;
+    DevBuf<unsigned char> d_work;        // the solver's workspace, device and host
+    std::vector<unsigned char> h_work;
+    void *sol = nullptr, *sol_params = nullptr;
     long long nr_m = 0;
     double nr_lmd = 0.0;
     bool nr_ready = false;
     bool nr_lost_to_bcpd = false;         // the non-rigid loop ended because cpd_bcpd_lowrank_begin took the low-rank factors
     // weighted E-step (BCPD): per-source exponent offsets (FP64 scratch, block minima, the float32 values the passes read) and
     // {log2 c, dead-column shift, la_min} for finalize 1; d_bc_es: {scale, sigma2, w} of a stand-alone cpd_bcpd_estep
-    float* d_la = nullptr;
-    double *d_la64 = nullptr, *d_la_part = nullptr, *d_bc_es = nullptr;
-    size_t la_cap = 0;
-    double* d_log2c = nullptr;
+    DevBuf<float> d_la;
+    DevBuf<double> d_la64, d_la_part, d_bc_es;
+    DevBuf<double> d_log2c;
     bool wgt_on = false;
     // BCPD registration loop (host_bcpd.inl): G^-1 (float32), the precision A and Sigma (FP64), all M x M in the internal order
-    BcpdState* d_bc = nullptr;
-    float* d_bc_ginv = nullptr;
-    double *d_bc_A = nullptr, *d_bc_S = nullptr, *d_bc_v = nullptr, *d_bc_r = nullptr, *d_bc_alpha = nullptr, *d_bc_sdiag = nullptr,
-           *d_bc_part = nullptr, *d_bc_sums = nullptr;
-    int64_t* d_bc_ipiv = nullptr;
-    int* d_bc_info = nullptr;             // [0] getrf's info, [1] getrs's
+    DevBuf<BcpdState> d_bc;
+    DevBuf<float> d_bc_ginv;
+    DevBuf<double> d_bc_A, d_bc_S, d_bc_v, d_bc_r, d_bc_alpha, d_bc_sdiag, d_bc_part, d_bc_sums;
+    DevBuf<int64_t> d_bc_ipiv;
+    DevBuf<int> d_bc_info;                // [0] getrf's info, [1] getrs's
     long long bc_m = 0;                   // source count the buffers were sized for
-    size_t bc_part_cap = 0;
     double bc_sigma2 = 0.0;               // host copy of the sigma2 the next E-step uses (culling decision)
     bool bc_ready = false;
     bool bc_stopped = false;              // a step failed (LU, sigma2): the loop needs a new cpd_bcpd_begin
-    cudaEvent_t bc_ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+    Event bc_ev[6];
     float bc_ms[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
-    long long bc_vec_m = 0, bc_dense_m = 0;   // source counts of the per-source vectors and of the three M x M buffers
     // low-rank mode (cpd_bcpd_lowrank_begin): the factor is the handle's low-rank Qt (d_lr_X); the K x K system and C = its
     // inverse, C Qt^T ([K][ld]), r in [3][m], w = C Rt (K x 3) and the pivots of the K x K LU
     bool bc_lowrank = false;
-    double *d_bc_sys = nullptr, *d_bc_C = nullptr, *d_bc_CQ = nullptr, *d_bc_rt = nullptr, *d_bc_w = nullptr;
-    int64_t* d_bc_lr_ipiv = nullptr;
-    long long bc_lr_m = 0;
-    int bc_lr_k = 0;
+    DevBuf<double> d_bc_sys, d_bc_C, d_bc_CQ, d_bc_rt, d_bc_w;
+    DevBuf<int64_t> d_bc_lr_ipiv;
     // GMMTree (host_gmmtree.inl, gmmtree.cuh): the tree (13 doubles per node) and its prepared form (16), per-point work arrays
-    // sized for gt_cap points (coordinates, sorted coordinates, 8 gammas, sort keys / values in and out, argmax), the run bounds
-    // of the keys, the chunk partials, the moments of a registration E-step and scratch
+    // (coordinates, sorted coordinates, 8 gammas, sort keys / values in and out, argmax), the run bounds of the keys, the chunk
+    // partials, the moments of a registration E-step and scratch
     int gt_levels = 0;                    // > 0: a tree is installed (cpd_gmmtree_build / cpd_gmmtree_load)
-    long long gt_total = 0, gt_cap = 0, gt_m = 0;   // nodes, point capacity, source count of the last build (0: loaded)
-    size_t gt_part_cap = 0, gt_sort_cap = 0;
-    double *d_gt_nodes = nullptr, *d_gt_prep = nullptr, *d_gt_pts = nullptr, *d_gt_spts = nullptr, *d_gt_g = nullptr,
-           *d_gt_part = nullptr, *d_gt_mom = nullptr, *d_gt_scr = nullptr;
-    unsigned *d_gt_keys = nullptr, *d_gt_keys2 = nullptr;
-    int *d_gt_idx = nullptr, *d_gt_idx2 = nullptr, *d_gt_cur = nullptr, *d_gt_start = nullptr, *d_gt_end = nullptr, *d_gt_asg = nullptr;
-    long long* d_gt_seeds = nullptr;
-    void* d_gt_sort = nullptr;
-    cudaEvent_t gt_ev[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+    long long gt_total = 0, gt_m = 0;     // nodes, source count of the last build (0: loaded)
+    DevBuf<double> d_gt_nodes, d_gt_prep, d_gt_pts, d_gt_spts, d_gt_g, d_gt_part, d_gt_mom, d_gt_scr;
+    DevBuf<unsigned> d_gt_keys, d_gt_keys2;
+    DevBuf<int> d_gt_idx, d_gt_idx2, d_gt_cur, d_gt_start, d_gt_end, d_gt_asg;
+    DevBuf<long long> d_gt_seeds;
+    DevBuf<unsigned char> d_gt_sort;
+    Event gt_ev[7];
     float gt_ms[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};   // build ms per level (up to 5), ms of the last registration E-step
     // correspondence priors of ConstrainedNonRigidCPD
-    double *d_wgt = nullptr, *d_p1t = nullptr, *d_pxt = nullptr;
+    DevBuf<double> d_wgt, d_p1t, d_pxt;
     long long prior_m = 0;
     double prior_alpha = 1.0;
     bool prior_on = false;
@@ -263,51 +339,40 @@ struct cpd_ctx {
     bool lr_w_stale = false;              // W of the low-rank path is formed on demand
     float lr_setup_ms[3] = {0.f, 0.f, 0.f};   // products / orthonormalisations / core of the last profiled set-up
     long long lr_m = 0;
-    int lr_cap = 0;
-    float4* d_lr_pts = nullptr;
-    double *d_lr_Q = nullptr, *d_lr_X = nullptr, *d_lr_coef = nullptr, *d_lr_part = nullptr, *d_lr_Bc = nullptr, *d_lr_S = nullptr,
-           *d_lr_R = nullptr, *d_lr_sys = nullptr, *d_lr_rhs = nullptr, *d_lr_c = nullptr, *d_lr_out = nullptr, *d_lr_panel = nullptr, *d_lr_Lt = nullptr;
+    DevBuf<float4> d_lr_pts;
+    DevBuf<double> d_lr_Q, d_lr_X, d_lr_coef, d_lr_part, d_lr_Bc, d_lr_S, d_lr_R, d_lr_sys, d_lr_rhs, d_lr_c, d_lr_out, d_lr_panel, d_lr_Lt;
     bool lr_spd = true;                   // symmetric positive definite K x K system on Qt = Q L (lr_spd_form); CPD_B200_LR_CORE=lu: LU of (c I + Bc S)
-    size_t lr_part_cap = 0;               // doubles in d_lr_part (slice partials of lr_inner)
-    unsigned char* d_gi_planes = nullptr;                      // exact int8-digit product: digit planes of X, FP64 chunk partials, column maxima
-    double *d_gi_part = nullptr, *d_gi_colmax = nullptr;
-    size_t gi_planes_cap = 0, gi_part_cap = 0, gi_colmax_cap = 0;
-    size_t lr_out_cap = 0;
-    P2PMailbox* d_box = nullptr;          // this rank's mailbox (peers write into it)
-    P2PInfo* d_p2p = nullptr;             // device copy of the peer table; non-null => fused P2P exchange
+    DevBuf<unsigned char> d_gi_planes;    // exact int8-digit product: digit planes of X, FP64 chunk partials, column maxima
+    DevBuf<double> d_gi_part, d_gi_colmax;
+    DevBuf<P2PMailbox> d_box;             // this rank's mailbox (peers write into it)
+    DevBuf<P2PInfo> d_p2p;                // device copy of the peer table; allocated => fused P2P exchange
     void* peer_ptr[P2P_MAX] = {nullptr};  // mappings opened with cudaIpcOpenMemHandle
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr, sev[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+    Event ev0, ev1, sev[7];
     bool profiling = false;
     int64_t launches = 0;
     // the fused EM iteration as a CUDA graph (cpd_em_step): one graph launch instead of 7-12 kernel launches per iteration
-    DevState* h_state_ring = nullptr;     // pinned staging slots of upload_state
-    cudaEvent_t state_ev[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+    PinBuf<DevState> h_state_ring;        // pinned staging slots of upload_state
+    Event state_ev[8];
     int state_slot = 0;
     bool graph_on = true;
-    cudaGraphExec_t em_graph = nullptr;
-    int em_graph_key = -1, em_graph_launches = 0, prepare_gen = 0;
-    void* d_flush = nullptr;
-    size_t flush_cap = 0;
-    std::vector<cudaEvent_t> pool;
+#ifndef CPD_HOST_EMU
+    GraphExec em_graph;                   // dropped whenever a buffer or peer table it captured changes (drop_graph)
+#endif
+    bool em_graph_cull = false;           // the culling choice em_graph was captured with
+    int em_graph_launches = 0;
+    DevBuf<unsigned char> d_flush;
+    std::vector<Event> pool;
 };
 
 namespace {
 constexpr int STATE_RING = 8;
-template <typename T>
-int dev_alloc(T** p, size_t count) {
-    if (*p) { cudaFree(*p); *p = nullptr; }
-    cudaError_t e = cudaMalloc((void**)p, std::max<size_t>(count, 1) * sizeof(T));
-    if (e != cudaSuccess) return fail(CPD_ERR_CUDA, "cudaMalloc(%zu bytes) failed: %s", count * sizeof(T), cudaGetErrorString(e));
-    return CPD_OK;
+// A captured EM graph replays the pointers it was captured with: it is dropped whenever one of them may change.
+inline void drop_graph(cpd_ctx* h) {
+#ifndef CPD_HOST_EMU
+    h->em_graph.reset();
+#endif
+    (void)h;
 }
-#define TRY(x) do { int r__ = (x); if (r__ != CPD_OK) return r__; } while (0)
-// device buffer of a stateless entry point: freed on every exit path
-template <typename T>
-struct DevBuf {
-    T* p = nullptr;
-    ~DevBuf() { if (p) cudaFree(p); }
-    int alloc(size_t count) { return dev_alloc(&p, count); }
-};
 
 inline unsigned blocks_for(long long n) { return (unsigned)((n + THREADS - 1) / THREADS); }
 
@@ -384,15 +449,15 @@ WorkList build_work(int ntiles, int nunits, int slots, double last_cost, double 
 int ensure_stats(cpd_ctx* h);
 int upload_state(cpd_ctx* h) {
     TRY(ensure_stats(h));
-    if (!h->h_state_ring) {
-        CU(cudaMallocHost((void**)&h->h_state_ring, STATE_RING * sizeof(DevState)));
-        for (int k = 0; k < STATE_RING; ++k) CU(cudaEventCreateWithFlags(&h->state_ev[k], cudaEventDisableTiming));
+    if (!h->h_state_ring.p) {
+        TRY(h->h_state_ring.alloc(STATE_RING));
+        for (Event& e : h->state_ev) CU(cudaEventCreateWithFlags(&e.e, cudaEventDisableTiming));
     }
     const int k = h->state_slot;
     h->state_slot = (k + 1) % STATE_RING;
     CU(cudaEventSynchronize(h->state_ev[k]));                  // never recorded: returns at once
-    h->h_state_ring[k] = h->h_state;
-    CU(cudaMemcpyAsync(h->d_state, &h->h_state_ring[k], sizeof(DevState), cudaMemcpyHostToDevice, h->stream));
+    h->h_state_ring.p[k] = h->h_state;
+    CU(cudaMemcpyAsync(h->d_state.p, &h->h_state_ring.p[k], sizeof(DevState), cudaMemcpyHostToDevice, h->stream));
     CU(cudaEventRecord(h->state_ev[k], h->stream));
     return CPD_OK;
 }
@@ -436,41 +501,30 @@ int cloud_sums_dev(cpd_ctx* h, const double* d_pts, long long count, double* par
 // consumed (copy_ev), so the caller's buffer is free again, as before.
 int ingest_cloud(cpd_ctx* h, const double* host_pts, long long count, int is_target, long long n_global, const double* origin,
                  int* d_perm, double* d_out) {
-    if (h->raw_cap < (size_t)count * 3) { TRY(dev_alloc(&h->d_raw, (size_t)count * 3)); h->raw_cap = (size_t)count * 3; }
+    TRY(h->d_raw.reserve((size_t)count * 3));
     const unsigned nb = blocks_for(count);
-    if (h->sums_cap < (size_t)nb * 9 + 16) {
-        TRY(dev_alloc(&h->d_sums, (size_t)nb * 9 + 16));
-        h->sums_cap = (size_t)nb * 9 + 16;
-    }
-    if (h->sort_cap < (size_t)count) {
-        TRY(dev_alloc(&h->d_codes, (size_t)count));
-        TRY(dev_alloc(&h->d_codes_out, (size_t)count));
-        TRY(dev_alloc(&h->d_idx_tmp, (size_t)count));
-        h->sort_cap = (size_t)count;
-    }
+    TRY(h->d_sums.reserve((size_t)nb * 9 + 16));
+    TRY(h->d_codes.reserve((size_t)count));
+    TRY(h->d_codes_out.reserve((size_t)count));
+    TRY(h->d_idx_tmp.reserve((size_t)count));
     size_t need = 0;
-    CU(cub::DeviceRadixSort::SortPairs(nullptr, need, h->d_codes, h->d_codes_out, h->d_idx_tmp, d_perm, (int)count, 0, 30, h->stream));
-    if (need > h->sort_tmp_cap) {
-        if (h->d_sort_tmp) cudaFree(h->d_sort_tmp);
-        h->d_sort_tmp = nullptr;
-        CU(cudaMalloc(&h->d_sort_tmp, need));
-        h->sort_tmp_cap = need;
-    }
-    TRY(upload_cloud(h, host_pts, count, h->d_raw));
+    CU(cub::DeviceRadixSort::SortPairs(nullptr, need, h->d_codes.p, h->d_codes_out.p, h->d_idx_tmp.p, d_perm, (int)count, 0, 30, h->stream));
+    TRY(h->d_sort_tmp.reserve(need));
+    TRY(upload_cloud(h, host_pts, count, h->d_raw.p));
     CU(cudaEventRecord(h->copy_ev, h->stream));
-    double* frame = h->d_frame + 8 * is_target;
-    stats_kernel<<<nb, THREADS, 0, h->stream>>>(h->d_raw, count, h->d_sums + 16);
-    stats_fold_kernel<<<1, 288, 0, h->stream>>>(h->d_sums + 16, (int)nb, h->d_sums);
-    cloud_frame_kernel<<<1, 32, 0, h->stream>>>(h->d_sums, count, is_target, n_global, origin != nullptr, origin ? origin[0] : 0.0,
-                                                origin ? origin[1] : 0.0, origin ? origin[2] : 0.0, h->d_state, frame);
-    CU(cudaMemcpyAsync(h->h_stats + 9 * is_target, h->d_sums, 9 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+    double* frame = h->d_frame.p + 8 * is_target;
+    stats_kernel<<<nb, THREADS, 0, h->stream>>>(h->d_raw.p, count, h->d_sums.p + 16);
+    stats_fold_kernel<<<1, 288, 0, h->stream>>>(h->d_sums.p + 16, (int)nb, h->d_sums.p);
+    cloud_frame_kernel<<<1, 32, 0, h->stream>>>(h->d_sums.p, count, is_target, n_global, origin != nullptr, origin ? origin[0] : 0.0,
+                                                origin ? origin[1] : 0.0, origin ? origin[2] : 0.0, h->d_state.p, frame);
+    CU(cudaMemcpyAsync(h->h_stats.p + 9 * is_target, h->d_sums.p, 9 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
     CU(cudaEventRecord(h->stats_ev, h->stream));
     h->stats_pending |= 1 << is_target;
     h->stats_count[is_target] = count;
-    morton_frame_kernel<<<nb, THREADS, 0, h->stream>>>(h->d_raw, count, frame, h->d_codes, h->d_idx_tmp);
-    CU(cub::DeviceRadixSort::SortPairs(h->d_sort_tmp, need, h->d_codes, h->d_codes_out, h->d_idx_tmp, d_perm, (int)count, 0, 30,
+    morton_frame_kernel<<<nb, THREADS, 0, h->stream>>>(h->d_raw.p, count, frame, h->d_codes.p, h->d_idx_tmp.p);
+    CU(cub::DeviceRadixSort::SortPairs(h->d_sort_tmp.p, need, h->d_codes.p, h->d_codes_out.p, h->d_idx_tmp.p, d_perm, (int)count, 0, 30,
                                        h->stream));
-    gather3_frame_kernel<<<nb, THREADS, 0, h->stream>>>(h->d_raw, d_perm, count, frame, d_out);
+    gather3_frame_kernel<<<nb, THREADS, 0, h->stream>>>(h->d_raw.p, d_perm, count, frame, d_out);
     KCHECK();
     h->launches += 6;
     CU(cudaEventSynchronize(h->copy_ev));
@@ -483,9 +537,9 @@ int ensure_stats(cpd_ctx* h) {
     if (!h->stats_pending) return CPD_OK;
     CU(cudaEventSynchronize(h->stats_ev));
     if (h->stats_pending & 1)
-        for (int a = 0; a < 3; ++a) h->h_state.cy[a] = h->h_stats[a] / (double)h->stats_count[0];
+        for (int a = 0; a < 3; ++a) h->h_state.cy[a] = h->h_stats.p[a] / (double)h->stats_count[0];
     if (h->stats_pending & 2) {
-        const double* t = h->h_stats + 9;
+        const double* t = h->h_stats.p + 9;
         if (!h->origin_given) for (int a = 0; a < 3; ++a) h->h_state.cx[a] = t[a] / (double)h->stats_count[1];
         h->extent = std::max(t[6] - t[3], std::max(t[7] - t[4], t[8] - t[5]));
     }
@@ -517,30 +571,30 @@ int prepare(cpd_ctx* h) {
     const WorkList w2 = build_work(h->it2, (int)(h->npad / P2_STAGE), h->slots2, 1.0, 0.5);
     h->j1 = w1.max_slots; h->g1 = (int)w1.items.size();
     h->j2 = w2.max_slots; h->g2 = (int)w2.items.size();
-    TRY(dev_alloc(&h->d_work1, w1.items.size()));
-    TRY(dev_alloc(&h->d_work2, w2.items.size()));
-    TRY(dev_alloc(&h->d_slots1, w1.tile_slots.size()));
-    TRY(dev_alloc(&h->d_slots2, w2.tile_slots.size()));
+    TRY(h->d_work1.alloc(w1.items.size()));
+    TRY(h->d_work2.alloc(w2.items.size()));
+    TRY(h->d_slots1.alloc(w1.tile_slots.size()));
+    TRY(h->d_slots2.alloc(w2.tile_slots.size()));
     // on the handle's (non-blocking) stream, which the consuming kernels run on; the vectors live until the synchronise below
-    CU(cudaMemcpyAsync(h->d_work1, w1.items.data(), w1.items.size() * sizeof(int4), cudaMemcpyHostToDevice, h->stream));
-    CU(cudaMemcpyAsync(h->d_work2, w2.items.data(), w2.items.size() * sizeof(int4), cudaMemcpyHostToDevice, h->stream));
-    CU(cudaMemcpyAsync(h->d_slots1, w1.tile_slots.data(), w1.tile_slots.size() * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-    CU(cudaMemcpyAsync(h->d_slots2, w2.tile_slots.data(), w2.tile_slots.size() * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    CU(cudaMemcpyAsync(h->d_work1.p, w1.items.data(), w1.items.size() * sizeof(int4), cudaMemcpyHostToDevice, h->stream));
+    CU(cudaMemcpyAsync(h->d_work2.p, w2.items.data(), w2.items.size() * sizeof(int4), cudaMemcpyHostToDevice, h->stream));
+    CU(cudaMemcpyAsync(h->d_slots1.p, w1.tile_slots.data(), w1.tile_slots.size() * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    CU(cudaMemcpyAsync(h->d_slots2.p, w2.tile_slots.data(), w2.tile_slots.size() * sizeof(int), cudaMemcpyHostToDevice, h->stream));
     CU(cudaStreamSynchronize(h->stream));
-    TRY(dev_alloc(&h->d_sbox, (size_t)(h->mpad / P1_STAGE) * 2));
-    TRY(dev_alloc(&h->d_tbox, (size_t)(h->npad / P2_STAGE) * 2));
-    TRY(dev_alloc(&h->d_omax, (size_t)(h->npad / P2_STAGE)));
-    TRY(dev_alloc(&h->d_ssub, (size_t)(h->mpad / SUB) * 2));
-    TRY(dev_alloc(&h->d_tsub, (size_t)(h->npad / SUB) * 2));
-    TRY(dev_alloc(&h->d_omax_sub, (size_t)(h->npad / SUB)));
+    TRY(h->d_sbox.alloc((size_t)(h->mpad / P1_STAGE) * 2));
+    TRY(h->d_tbox.alloc((size_t)(h->npad / P2_STAGE) * 2));
+    TRY(h->d_omax.alloc((size_t)(h->npad / P2_STAGE)));
+    TRY(h->d_ssub.alloc((size_t)(h->mpad / SUB) * 2));
+    TRY(h->d_tsub.alloc((size_t)(h->npad / SUB) * 2));
+    TRY(h->d_omax_sub.alloc((size_t)(h->npad / SUB)));
     const size_t need1 = (size_t)h->j1 * h->n, need2 = (size_t)h->j2 * h->m * 4;
-    if (need1 > h->part1_cap) { TRY(dev_alloc(&h->d_part1, need1)); h->part1_cap = need1; }
-    if (need2 > h->part2_cap) { TRY(dev_alloc(&h->d_part2, need2)); h->part2_cap = need2; }
+    TRY(h->d_part1.reserve(need1));
+    TRY(h->d_part2.reserve(need2));
     const size_t ms = (size_t)blocks_for(h->m) * MOM_SRC, mt = (size_t)blocks_for(h->npad) * MOM_TGT;   // MOM_* >= RM_*
-    if (ms > h->mom_src_cap) { TRY(dev_alloc(&h->d_mom_src, ms)); h->mom_src_cap = ms; }
-    if (mt > h->mom_tgt_cap) { TRY(dev_alloc(&h->d_mom_tgt, mt)); h->mom_tgt_cap = mt; }
+    TRY(h->d_mom_src.reserve(ms));
+    TRY(h->d_mom_tgt.reserve(mt));
     h->prepared = true;
-    h->prepare_gen += 1;                 // buffers / work lists changed: a captured EM graph is stale
+    drop_graph(h);
     return CPD_OK;
 }
 
@@ -559,46 +613,46 @@ int launch_estep(cpd_ctx* h, const double* d_sigma2, const double* d_w, const do
     TRY(prepare(h));
     const long long cover = std::max(h->mpad, h->n);
     mark(h, 0);
-    pack_kernel<<<blocks_for(cover), THREADS, 0, h->stream>>>(h->d_state, d_sigma2, h->d_yc, d_ts, h->d_xc, h->m, h->mpad,
-                                                              h->n, h->d_srcP, h->d_tgtP);
+    pack_kernel<<<blocks_for(cover), THREADS, 0, h->stream>>>(h->d_state.p, d_sigma2, h->d_yc.p, d_ts, h->d_xc.p, h->m, h->mpad,
+                                                              h->n, h->d_srcP.p, h->d_tgtP.p);
     mark(h, 1);
     const bool cull = h->cull_on && h->cull_active;
     const int nst1 = (int)(h->mpad / P1_STAGE);
-    stage_bbox_kernel<<<(unsigned)nst1, THREADS, 0, h->stream>>>(h->d_srcP, (int)h->m, P1_STAGE, h->d_sbox);   // offset seeding (always)
+    stage_bbox_kernel<<<(unsigned)nst1, THREADS, 0, h->stream>>>(h->d_srcP.p, (int)h->m, P1_STAGE, h->d_sbox.p);   // offset seeding (always)
     h->launches += 1;
     const int nsub1 = (int)(h->mpad / SUB), nsub2 = (int)(h->npad / SUB);
     if (cull) {
-        stage_bbox_kernel<<<(unsigned)(h->npad / P2_STAGE), THREADS, 0, h->stream>>>(h->d_tgtP, (int)h->n, P2_STAGE, h->d_tbox);
-        sub_bbox_kernel<<<(unsigned)((nsub1 + 7) / 8), THREADS, 0, h->stream>>>(h->d_srcP, (int)h->m, nsub1, h->d_ssub);
-        sub_bbox_kernel<<<(unsigned)((nsub2 + 7) / 8), THREADS, 0, h->stream>>>(h->d_tgtP, (int)h->n, nsub2, h->d_tsub);
+        stage_bbox_kernel<<<(unsigned)(h->npad / P2_STAGE), THREADS, 0, h->stream>>>(h->d_tgtP.p, (int)h->n, P2_STAGE, h->d_tbox.p);
+        sub_bbox_kernel<<<(unsigned)((nsub1 + 7) / 8), THREADS, 0, h->stream>>>(h->d_srcP.p, (int)h->m, nsub1, h->d_ssub.p);
+        sub_bbox_kernel<<<(unsigned)((nsub2 + 7) / 8), THREADS, 0, h->stream>>>(h->d_tgtP.p, (int)h->n, nsub2, h->d_tsub.p);
         h->launches += 3;
     }
     const bool wgt = h->wgt_on;
     if (wgt) {
-        weight_patch_kernel<<<blocks_for(h->m), THREADS, 0, h->stream>>>(h->d_la, h->m, h->d_srcP);
+        weight_patch_kernel<<<blocks_for(h->m), THREADS, 0, h->stream>>>(h->d_la.p, h->m, h->d_srcP.p);
         h->launches += 1;
     }
-#define CPD_PASS1(C, W) pass1_kernel<C, W><<<h->g1, THREADS, PASS1_SMEM, h->stream>>>(h->d_tgtP, (int)h->n, h->d_srcP, h->d_work1, h->d_part1, h->d_sbox, nst1, (C) ? h->d_ssub : nullptr)
+#define CPD_PASS1(C, W) pass1_kernel<C, W><<<h->g1, THREADS, PASS1_SMEM, h->stream>>>(h->d_tgtP.p, (int)h->n, h->d_srcP.p, h->d_work1.p, h->d_part1.p, h->d_sbox.p, nst1, (C) ? h->d_ssub.p : nullptr)
     if (cull) { if (wgt) CPD_PASS1(true, true); else CPD_PASS1(true, false); }
     else { if (wgt) CPD_PASS1(false, true); else CPD_PASS1(false, false); }
 #undef CPD_PASS1
     mark(h, 2);
-    finalize1_kernel<<<blocks_for(h->npad), THREADS, 0, h->stream>>>(h->d_state, d_sigma2, d_w, h->d_part1, h->d_slots1, (int)h->n,
-                                                                     h->d_tgtP, h->d_tgtQ, h->npad, h->d_pt1, h->d_mom_tgt,
-                                                                     wgt ? h->d_log2c : nullptr);
+    finalize1_kernel<<<blocks_for(h->npad), THREADS, 0, h->stream>>>(h->d_state.p, d_sigma2, d_w, h->d_part1.p, h->d_slots1.p, (int)h->n,
+                                                                     h->d_tgtP.p, h->d_tgtQ.p, h->npad, h->d_pt1.p, h->d_mom_tgt.p,
+                                                                     wgt ? h->d_log2c.p : nullptr);
     mark(h, 3);
     if (cull) {
-        stage_omax_kernel<<<(unsigned)(h->npad / P2_STAGE), THREADS, 0, h->stream>>>(h->d_tgtQ, h->d_omax);
-        sub_omax_kernel<<<(unsigned)((nsub2 + 7) / 8), THREADS, 0, h->stream>>>(h->d_tgtQ, nsub2, h->d_omax_sub);
+        stage_omax_kernel<<<(unsigned)(h->npad / P2_STAGE), THREADS, 0, h->stream>>>(h->d_tgtQ.p, h->d_omax.p);
+        sub_omax_kernel<<<(unsigned)((nsub2 + 7) / 8), THREADS, 0, h->stream>>>(h->d_tgtQ.p, nsub2, h->d_omax_sub.p);
         h->launches += 2;
     }
-#define CPD_PASS2(C, W) pass2_kernel<C, W><<<h->g2, THREADS, PASS2_SMEM, h->stream>>>(h->d_srcP, (int)h->m, h->d_tgtQ, h->d_work2, h->d_part2, (C) ? h->d_tbox : nullptr, (C) ? h->d_omax : nullptr, (C) ? h->d_tsub : nullptr, (C) ? h->d_omax_sub : nullptr)
+#define CPD_PASS2(C, W) pass2_kernel<C, W><<<h->g2, THREADS, PASS2_SMEM, h->stream>>>(h->d_srcP.p, (int)h->m, h->d_tgtQ.p, h->d_work2.p, h->d_part2.p, (C) ? h->d_tbox.p : nullptr, (C) ? h->d_omax.p : nullptr, (C) ? h->d_tsub.p : nullptr, (C) ? h->d_omax_sub.p : nullptr)
     if (cull) { if (wgt) CPD_PASS2(true, true); else CPD_PASS2(true, false); }
     else { if (wgt) CPD_PASS2(false, true); else CPD_PASS2(false, false); }
 #undef CPD_PASS2
     mark(h, 4);
-    finalize2_kernel<<<blocks_for(h->m), THREADS, 0, h->stream>>>(h->d_state, d_sigma2, h->d_part2, h->d_slots2, (int)h->m, h->d_yc,
-                                                                  d_ts, h->d_p1, h->d_pxc, h->d_mom_src);
+    finalize2_kernel<<<blocks_for(h->m), THREADS, 0, h->stream>>>(h->d_state.p, d_sigma2, h->d_part2.p, h->d_slots2.p, (int)h->m, h->d_yc.p,
+                                                                  d_ts, h->d_p1.p, h->d_pxc.p, h->d_mom_src.p);
     mark(h, 5);
     mark(h, 6);          // E-step-only callers end here; cpd_em_step / cpd_nonrigid_step record event 6 again after their M-step
     KCHECK();
@@ -607,23 +661,23 @@ int launch_estep(cpd_ctx* h, const double* d_sigma2, const double* d_w, const do
 }
 
 int read_params(cpd_ctx* h, cpd_params* out) {
-    static_assert(sizeof(DevState) <= 48 * sizeof(double), "DevState outgrew the pinned staging buffer");
-    CU(cudaMemcpyAsync(h->h_pin, h->d_state, sizeof(DevState), cudaMemcpyDeviceToHost, h->stream));
+    const DevState& s = h->pin.p->state;
+    CU(cudaMemcpyAsync(&h->pin.p->state, h->d_state.p, sizeof(DevState), cudaMemcpyDeviceToHost, h->stream));
     CU(cudaStreamSynchronize(h->stream));
-    if (reinterpret_cast<const DevState*>(h->h_pin)->err)
+    if (s.err)
         return fail(CPD_ERR_STATE, "a peer rank did not deliver its moments within the P2P exchange timeout");
     const int d = h->dim;
     for (int i = 0; i < 9; ++i) out->lin[i] = 0.0;
     for (int i = 0; i < d; ++i)
-        for (int j = 0; j < d; ++j) out->lin[i * d + j] = h->h_pin[3 * i + j];
-    for (int i = 0; i < 3; ++i) out->t[i] = (i < d) ? h->h_pin[9 + i] : 0.0;
-    out->scale = h->h_pin[12];
-    out->sigma2 = h->h_pin[13];
+        for (int j = 0; j < d; ++j) out->lin[i * d + j] = s.lin[3 * i + j];
+    for (int i = 0; i < 3; ++i) out->t[i] = (i < d) ? s.t[i] : 0.0;
+    out->scale = s.scale;
+    out->sigma2 = s.sigma2;
     // a point reaches ~13.3 sigma (2^-127); culling can only pay once that is well inside the cloud
     TRY(ensure_stats(h));
     h->cull_active = h->extent > 0.0 && 13.3 * sqrt(out->sigma2) < 0.25 * h->extent;
-    out->q = h->h_pin[14];
-    out->n_p = h->h_pin[15];
+    out->q = s.q;
+    out->n_p = s.n_p;
     return CPD_OK;
 }
 }  // namespace
@@ -660,12 +714,12 @@ extern "C" int cpd_create(cpd_ctx** out, int device, int dim, void* stream) {
     CU(cudaGetDeviceProperties(&prop, device));
     if (prop.major != 9 || prop.minor != 0)
         return fail(CPD_ERR_CUDA, "device %d is sm_%d%d; this library is built for sm_90a (Hopper) only", device, prop.major, prop.minor);
-    cpd_ctx* h = new cpd_ctx();
+    std::unique_ptr<cpd_ctx> h(new cpd_ctx());
     h->device = device;
     h->dim = dim;
     h->sm_count = prop.multiProcessorCount;
-    if (stream) { h->stream = (cudaStream_t)stream; h->own_stream = false; }
-    else { CU(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking)); h->own_stream = true; }
+    if (stream) h->stream = (cudaStream_t)stream;
+    else { CU(cudaStreamCreateWithFlags(&h->owned_stream.s, cudaStreamNonBlocking)); h->stream = h->owned_stream.s; }
     CU(cudaFuncSetAttribute(pass1_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, PASS1_SMEM));
     CU(cudaFuncSetAttribute(pass2_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, PASS2_SMEM));
     CU(cudaFuncSetAttribute(pass1_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, PASS1_SMEM));
@@ -679,16 +733,16 @@ extern "C" int cpd_create(cpd_ctx** out, int device, int dim, void* stream) {
     CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ2, pass2_kernel<false, false>, THREADS, PASS2_SMEM));
     h->slots1 = h->sm_count * std::max(1, occ1);
     h->slots2 = h->sm_count * std::max(1, occ2);
-    TRY(dev_alloc(&h->d_state, 1));
-    TRY(dev_alloc(&h->d_mom, (size_t)MOM_PAD));
-    CU(cudaMallocHost((void**)&h->h_pin, 64 * sizeof(double)));
-    TRY(dev_alloc(&h->d_frame, 16));
-    CU(cudaMallocHost((void**)&h->h_stats, 18 * sizeof(double)));
-    CU(cudaEventCreateWithFlags(&h->stats_ev, cudaEventDisableTiming));
-    CU(cudaEventCreateWithFlags(&h->copy_ev, cudaEventDisableTiming));
-    CU(cudaEventCreate(&h->ev0));
-    CU(cudaEventCreate(&h->ev1));
-    for (int k = 0; k < 7; ++k) CU(cudaEventCreate(&h->sev[k]));
+    TRY(h->d_state.alloc(1));
+    TRY(h->d_mom.alloc((size_t)MOM_PAD));
+    TRY(h->pin.alloc(1));
+    TRY(h->d_frame.alloc(16));
+    TRY(h->h_stats.alloc(18));
+    CU(cudaEventCreateWithFlags(&h->stats_ev.e, cudaEventDisableTiming));
+    CU(cudaEventCreateWithFlags(&h->copy_ev.e, cudaEventDisableTiming));
+    CU(cudaEventCreate(&h->ev0.e));
+    CU(cudaEventCreate(&h->ev1.e));
+    for (Event& e : h->sev) CU(cudaEventCreate(&e.e));
     { const char* e = getenv("CPD_B200_NO_CULL"); h->cull_on = !(e && e[0] == '1'); }
     { const char* e = getenv("CPD_B200_NO_GRAPH"); h->graph_on = !(e && e[0] == '1'); }
     memset(&h->h_state, 0, sizeof(DevState));
@@ -696,78 +750,40 @@ extern "C" int cpd_create(cpd_ctx** out, int device, int dim, void* stream) {
     h->h_state.scale = 1.0;
     h->h_state.lin[0] = h->h_state.lin[4] = h->h_state.lin[8] = 1.0;
     h->h_state.update_scale = 1;
-    *out = h;
-    return upload_state(h);          // the device state starts as a copy of the host's (cloud_frame_kernel patches single fields)
+    TRY(upload_state(h.get()));      // the device state starts as a copy of the host's (cloud_frame_kernel patches single fields)
+    *out = h.release();
+    return CPD_OK;
 }
 
 extern "C" void cpd_destroy(cpd_ctx* h) {
     if (!h) return;
     cudaSetDevice(h->device);
     cudaStreamSynchronize(h->stream);
-    void* wl[] = {h->d_work1, h->d_work2, h->d_slots1, h->d_slots2, h->d_sbox, h->d_tbox, h->d_omax, h->d_ssub, h->d_tsub, h->d_omax_sub};
-    for (void* p : wl) if (p) cudaFree(p);
-    void* srt[] = {h->d_perm_src, h->d_perm_tgt, h->d_idx_tmp, h->d_codes, h->d_codes_out, h->d_sort_tmp, h->d_outN, h->d_outM};
-    for (void* p : srt) if (p) cudaFree(p);
-    void* nrp[] = {h->d_G, h->d_W, h->d_A, h->d_B, h->d_ts2, h->d_nrpart, h->d_ipiv, h->d_info, h->d_work};
-    for (void* p : nrp) if (p) cudaFree(p);
-    void* lrp[] = {h->d_lr_pts, h->d_lr_Q, h->d_lr_X, h->d_lr_coef, h->d_lr_part, h->d_lr_Bc, h->d_lr_S, h->d_lr_R, h->d_lr_sys, h->d_lr_rhs,
-                   h->d_lr_c, h->d_lr_out, h->d_lr_panel, h->d_lr_Lt, h->d_gi_planes, h->d_gi_part, h->d_gi_colmax, h->d_wgt, h->d_p1t, h->d_pxt, h->d_la, h->d_log2c,
-                   h->d_la64, h->d_la_part, h->d_bc_es};
-    for (void* p : lrp) if (p) cudaFree(p);
-    void* bcp[] = {h->d_bc, h->d_bc_ginv, h->d_bc_A, h->d_bc_S, h->d_bc_v, h->d_bc_r, h->d_bc_alpha, h->d_bc_sdiag, h->d_bc_part, h->d_bc_sums,
-                   h->d_bc_ipiv, h->d_bc_info, h->d_bc_sys, h->d_bc_C, h->d_bc_CQ, h->d_bc_rt, h->d_bc_w, h->d_bc_lr_ipiv};
-    for (void* p : bcp) if (p) cudaFree(p);
-    for (cudaEvent_t e : h->bc_ev) if (e) cudaEventDestroy(e);
-    void* gtp[] = {h->d_gt_nodes, h->d_gt_prep, h->d_gt_pts, h->d_gt_spts, h->d_gt_g, h->d_gt_part, h->d_gt_mom, h->d_gt_scr, h->d_gt_keys,
-                   h->d_gt_keys2, h->d_gt_idx, h->d_gt_idx2, h->d_gt_cur, h->d_gt_start, h->d_gt_end, h->d_gt_asg, h->d_gt_seeds, h->d_gt_sort};
-    for (void* p : gtp) if (p) cudaFree(p);
-    for (cudaEvent_t e : h->gt_ev) if (e) cudaEventDestroy(e);
-    if (h->h_work) free(h->h_work);
+    for (void* p : h->peer_ptr) if (p) cudaIpcCloseMemHandle(p);
     if (h->sol_params && g_sol.DestroyParams) g_sol.DestroyParams(h->sol_params);
     if (h->sol && g_sol.Destroy) g_sol.Destroy(h->sol);
-    for (int r = 0; r < P2P_MAX; ++r) if (h->peer_ptr[r]) cudaIpcCloseMemHandle(h->peer_ptr[r]);
-    if (h->d_box) cudaFree(h->d_box);
-    if (h->d_p2p) cudaFree(h->d_p2p);
-    void* ptrs[] = {h->d_yc, h->d_ts, h->d_xc, h->d_raw, h->d_srcP, h->d_tgtP, h->d_tgtQ, h->d_part1, h->d_part2, h->d_pt1, h->d_p1,
-                    h->d_pxc, h->d_px, h->d_mom_src, h->d_mom_tgt, h->d_mom, h->d_sums, h->d_state, h->d_flush};
-    for (void* p : ptrs) if (p) cudaFree(p);
-    if (h->h_pin) cudaFreeHost(h->h_pin);
-    if (h->h_stats) cudaFreeHost(h->h_stats);
-    if (h->d_frame) cudaFree(h->d_frame);
-    if (h->stats_ev) cudaEventDestroy(h->stats_ev);
-    if (h->copy_ev) cudaEventDestroy(h->copy_ev);
-#ifndef CPD_HOST_EMU
-    if (h->em_graph) cudaGraphExecDestroy(h->em_graph);
-#endif
-    if (h->h_state_ring) cudaFreeHost(h->h_state_ring);
-    for (int k = 0; k < 8; ++k) if (h->state_ev[k]) cudaEventDestroy(h->state_ev[k]);
-    if (h->ev0) cudaEventDestroy(h->ev0);
-    if (h->ev1) cudaEventDestroy(h->ev1);
-    for (int k = 0; k < 7; ++k) if (h->sev[k]) cudaEventDestroy(h->sev[k]);
-    for (cudaEvent_t e : h->pool) if (e) cudaEventDestroy(e);
-    if (h->own_stream) cudaStreamDestroy(h->stream);
-    delete h;
+    delete h;                        // every buffer, pinned block, event and graph; the stream the handle created last
 }
 
 extern "C" int cpd_set_source(cpd_ctx* h, const double* source, int64_t m) {
     if (!h || !source) return fail(CPD_ERR_ARG, "null argument");
     if (m < 1 || m > 0x7fffffffLL - 65536) return fail(CPD_ERR_ARG, "source count %lld out of range", (long long)m);
     CU(cudaSetDevice(h->device));
-    if (m != h->m || !h->d_yc) {
+    if (m != h->m || !h->d_yc.p) {
         h->m = m;
         h->mpad = (m + P1_STAGE - 1) / P1_STAGE * P1_STAGE;
-        TRY(dev_alloc(&h->d_yc, (size_t)m * 3));
-        TRY(dev_alloc(&h->d_ts, (size_t)m * 3));
-        TRY(dev_alloc(&h->d_srcP, (size_t)h->mpad));
-        TRY(dev_alloc(&h->d_p1, (size_t)m));
-        TRY(dev_alloc(&h->d_pxc, (size_t)m * 3));
-        TRY(dev_alloc(&h->d_px, (size_t)m * 3));
-        TRY(dev_alloc(&h->d_perm_src, (size_t)m));
-        TRY(dev_alloc(&h->d_outM, (size_t)m * 3));
+        TRY(h->d_yc.alloc((size_t)m * 3));
+        TRY(h->d_ts.alloc((size_t)m * 3));
+        TRY(h->d_srcP.alloc((size_t)h->mpad));
+        TRY(h->d_p1.alloc((size_t)m));
+        TRY(h->d_pxc.alloc((size_t)m * 3));
+        TRY(h->d_px.alloc((size_t)m * 3));
+        TRY(h->d_perm_src.alloc((size_t)m));
+        TRY(h->d_outM.alloc((size_t)m * 3));
         h->prepared = false;
         h->nr_ready = false;
     }
-    TRY(ingest_cloud(h, source, m, 0, 0, nullptr, h->d_perm_src, h->d_yc));
+    TRY(ingest_cloud(h, source, m, 0, 0, nullptr, h->d_perm_src.p, h->d_yc.p));
     h->bc_ready = false;                 // a BCPD loop starts from its own cpd_set_source + cpd_bcpd_begin
     h->bc_stopped = false;
     h->h_state.m = m;
@@ -781,15 +797,15 @@ extern "C" int cpd_set_target(cpd_ctx* h, const double* target, int64_t n_local,
     if (n_global < n_local) return fail(CPD_ERR_ARG, "n_global (%lld) < n_local (%lld)", (long long)n_global, (long long)n_local);
     if (!frame_origin && n_global != n_local) return fail(CPD_ERR_ARG, "a sharded target needs an explicit frame_origin");
     CU(cudaSetDevice(h->device));
-    if (n_local != h->n || !h->d_xc) {
+    if (n_local != h->n || !h->d_xc.p) {
         h->n = n_local;
         h->npad = (n_local + P2_STAGE - 1) / P2_STAGE * P2_STAGE;
-        TRY(dev_alloc(&h->d_xc, (size_t)n_local * 3));
-        TRY(dev_alloc(&h->d_tgtP, (size_t)n_local));
-        TRY(dev_alloc(&h->d_tgtQ, (size_t)h->npad * 2));
-        TRY(dev_alloc(&h->d_pt1, (size_t)n_local));
-        TRY(dev_alloc(&h->d_perm_tgt, (size_t)n_local));
-        TRY(dev_alloc(&h->d_outN, (size_t)n_local));
+        TRY(h->d_xc.alloc((size_t)n_local * 3));
+        TRY(h->d_tgtP.alloc((size_t)n_local));
+        TRY(h->d_tgtQ.alloc((size_t)h->npad * 2));
+        TRY(h->d_pt1.alloc((size_t)n_local));
+        TRY(h->d_perm_tgt.alloc((size_t)n_local));
+        TRY(h->d_outN.alloc((size_t)n_local));
         h->prepared = false;
     }
     h->n_global = n_global;
@@ -797,7 +813,7 @@ extern "C" int cpd_set_target(cpd_ctx* h, const double* target, int64_t n_local,
     if (frame_origin) for (int a = 0; a < h->dim; ++a) origin[a] = frame_origin[a];
     h->origin_given = frame_origin != nullptr;
     if (h->origin_given) for (int a = 0; a < 3; ++a) h->h_state.cx[a] = origin[a];
-    TRY(ingest_cloud(h, target, n_local, 1, n_global, frame_origin ? origin : nullptr, h->d_perm_tgt, h->d_xc));
+    TRY(ingest_cloud(h, target, n_local, 1, n_global, frame_origin ? origin : nullptr, h->d_perm_tgt.p, h->d_xc.p));
     h->h_state.n_global = n_global;
     h->have_target = true;
     return CPD_OK;
@@ -810,14 +826,14 @@ extern "C" int cpd_sigma2_init(cpd_ctx* h, double* sigma2) {
     // target sums (summed over the ranks on the device), source sums, ONE read-back: a single host synchronisation
     double sx[4], sy[4];
     const size_t pn = (size_t)blocks_for(h->n) * 4, pm = (size_t)blocks_for(h->m) * 4;
-    if (h->sums_cap < 16 + pn + pm) { TRY(dev_alloc(&h->d_sums, 16 + pn + pm)); h->sums_cap = 16 + pn + pm; }
-    TRY(cloud_sums_dev(h, h->d_xc, h->n, h->d_sums + 16, h->d_sums));
-    if (h->comm) TRY(allreduce(h, h->d_sums, 4));
-    TRY(cloud_sums_dev(h, h->d_yc, h->m, h->d_sums + 16 + pn, h->d_sums + 4));
-    CU(cudaMemcpyAsync(h->h_pin, h->d_sums, 8 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+    TRY(h->d_sums.reserve(16 + pn + pm));
+    TRY(cloud_sums_dev(h, h->d_xc.p, h->n, h->d_sums.p + 16, h->d_sums.p));
+    if (h->comm) TRY(allreduce(h, h->d_sums.p, 4));
+    TRY(cloud_sums_dev(h, h->d_yc.p, h->m, h->d_sums.p + 16 + pn, h->d_sums.p + 4));
+    CU(cudaMemcpyAsync(h->pin.p->sums, h->d_sums.p, 8 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
     CU(cudaStreamSynchronize(h->stream));
     TRY(ensure_stats(h));
-    for (int k = 0; k < 4; ++k) { sx[k] = h->h_pin[k]; sy[k] = h->h_pin[4 + k]; }
+    for (int k = 0; k < 4; ++k) { sx[k] = h->pin.p->sums[k]; sy[k] = h->pin.p->sums[4 + k]; }
     // move the source sums into the targets' frame: y' = y~ + (cy - cx)
     double dlt[3], d2 = 0.0, dsy = 0.0;
     for (int a = 0; a < 3; ++a) { dlt[a] = h->h_state.cy[a] - h->h_state.cx[a]; d2 += dlt[a] * dlt[a]; dsy += dlt[a] * sy[1 + a]; }
@@ -857,19 +873,19 @@ extern "C" int cpd_set_state(cpd_ctx* h, int tf_kind, int update_scale, double w
 namespace {
 // the launches of one fused EM iteration, in stream order (also what a graph capture records)
 int em_step_launches(cpd_ctx* h) {
-    TRY(launch_estep(h, &h->d_state->sigma2, &h->d_state->w, nullptr));
+    TRY(launch_estep(h, &h->d_state.p->sigma2, &h->d_state.p->w, nullptr));
     const int nbs = (int)blocks_for(h->m), nbt = (int)blocks_for(h->npad);
-    if (h->d_p2p) {
-        moments_p2p_kernel<<<1, 256, 0, h->stream>>>(h->d_state, h->d_mom_src, nbs, RM_SRC, h->d_mom_tgt, nbt, RM_TGT, h->d_mom,
-                                                     h->d_p2p);
+    if (h->d_p2p.p) {
+        moments_p2p_kernel<<<1, 256, 0, h->stream>>>(h->d_state.p, h->d_mom_src.p, nbs, RM_SRC, h->d_mom_tgt.p, nbt, RM_TGT, h->d_mom.p,
+                                                     h->d_p2p.p);
         h->launches += 1;
     } else if (h->comm) {
-        moments_kernel<0><<<1, 256, 0, h->stream>>>(h->d_state, h->d_mom_src, nbs, RM_SRC, h->d_mom_tgt, nbt, RM_TGT, h->d_mom);
-        TRY(allreduce(h, h->d_mom, MOM_PAD));
-        mstep_residual_kernel<<<1, 32, 0, h->stream>>>(h->d_state, h->d_mom);
+        moments_kernel<0><<<1, 256, 0, h->stream>>>(h->d_state.p, h->d_mom_src.p, nbs, RM_SRC, h->d_mom_tgt.p, nbt, RM_TGT, h->d_mom.p);
+        TRY(allreduce(h, h->d_mom.p, MOM_PAD));
+        mstep_residual_kernel<<<1, 32, 0, h->stream>>>(h->d_state.p, h->d_mom.p);
         h->launches += 2;
     } else {
-        moments_kernel<1><<<1, 256, 0, h->stream>>>(h->d_state, h->d_mom_src, nbs, RM_SRC, h->d_mom_tgt, nbt, RM_TGT, h->d_mom);
+        moments_kernel<1><<<1, 256, 0, h->stream>>>(h->d_state.p, h->d_mom_src.p, nbs, RM_SRC, h->d_mom_tgt.p, nbt, RM_TGT, h->d_mom.p);
         h->launches += 1;
     }
     mark(h, 6);
@@ -886,7 +902,7 @@ extern "C" int cpd_em_step(cpd_ctx* h, cpd_params* out) {
     if (!h->have_state) return fail(CPD_ERR_STATE, "cpd_set_state has not been called");
     CU(cudaSetDevice(h->device));
 #ifndef CPD_HOST_EMU
-    const bool use_graph = h->graph_on && !h->profiling && !(h->comm && !h->d_p2p) && !h->wgt_on;
+    const bool use_graph = h->graph_on && !h->profiling && !(h->comm && !h->d_p2p.p) && !h->wgt_on;
 #else
     const bool use_graph = false;
 #endif
@@ -896,9 +912,9 @@ extern "C" int cpd_em_step(cpd_ctx* h, cpd_params* out) {
 #ifndef CPD_HOST_EMU
     else {
         TRY(prepare(h));                                    // allocations and uploads happen outside the capture
-        const int key = h->prepare_gen * 2 + ((h->cull_on && h->cull_active) ? 1 : 0);
-        if (!h->em_graph || h->em_graph_key != key) {
-            if (h->em_graph) { cudaGraphExecDestroy(h->em_graph); h->em_graph = nullptr; }
+        const bool cull = h->cull_on && h->cull_active;
+        if (!h->em_graph || h->em_graph_cull != cull) {
+            h->em_graph.reset();
             const int64_t before = h->launches;
             cudaGraph_t g = nullptr;
             CU(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));
@@ -908,12 +924,14 @@ extern "C" int cpd_em_step(cpd_ctx* h, cpd_params* out) {
             h->launches = before;
             if (rc != CPD_OK) { if (g) cudaGraphDestroy(g); return rc; }
             if (ce != cudaSuccess) return fail(CPD_ERR_CUDA, "cudaStreamEndCapture failed: %s", cudaGetErrorString(ce));
-            const cudaError_t ie = cudaGraphInstantiate(&h->em_graph, g, 0);
+            cudaGraphExec_t exec = nullptr;
+            const cudaError_t ie = cudaGraphInstantiate(&exec, g, 0);
             cudaGraphDestroy(g);
-            if (ie != cudaSuccess) { h->em_graph = nullptr; return fail(CPD_ERR_CUDA, "cudaGraphInstantiate failed: %s", cudaGetErrorString(ie)); }
-            h->em_graph_key = key;
+            if (ie != cudaSuccess) return fail(CPD_ERR_CUDA, "cudaGraphInstantiate failed: %s", cudaGetErrorString(ie));
+            h->em_graph.reset(exec);
+            h->em_graph_cull = cull;
         }
-        CU(cudaGraphLaunch(h->em_graph, h->stream));
+        CU(cudaGraphLaunch(h->em_graph.get(), h->stream));
         h->launches += h->em_graph_launches;                // kernels executed, whatever carried them to the device
     }
 #endif
@@ -946,19 +964,19 @@ extern "C" int cpd_estep(cpd_ctx* h, const double* t_source, double sigma2, doub
     if (!(w >= 0.0 && w < 1.0)) return fail(CPD_ERR_ARG, "w must be in [0, 1), got %g", w);
     if (!h->have_source || !h->have_target) return fail(CPD_ERR_STATE, "source and target must both be set");
     CU(cudaSetDevice(h->device));
-    if (h->raw_cap < (size_t)h->m * 3) { TRY(dev_alloc(&h->d_raw, (size_t)h->m * 3)); h->raw_cap = (size_t)h->m * 3; }
-    TRY(upload_cloud(h, t_source, h->m, h->d_raw));
-    gather3_kernel<<<blocks_for(h->m), THREADS, 0, h->stream>>>(h->d_raw, h->d_perm_src, h->m, 0.0, 0.0, 0.0, h->d_ts);
+    TRY(h->d_raw.reserve((size_t)h->m * 3));
+    TRY(upload_cloud(h, t_source, h->m, h->d_raw.p));
+    gather3_kernel<<<blocks_for(h->m), THREADS, 0, h->stream>>>(h->d_raw.p, h->d_perm_src.p, h->m, 0.0, 0.0, 0.0, h->d_ts.p);
     h->launches += 1;
     TRY(ensure_stats(h));
     h->cull_active = h->extent > 0.0 && 13.3 * sqrt(sigma2) < 0.25 * h->extent;
-    h->h_pin[32] = sigma2;
-    h->h_pin[33] = w;
-    CU(cudaMemcpyAsync(&h->d_state->es_sigma2, h->h_pin + 32, 2 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-    TRY(launch_estep(h, &h->d_state->es_sigma2, &h->d_state->es_w, h->d_ts));
+    h->pin.p->es[0] = sigma2;
+    h->pin.p->es[1] = w;
+    CU(cudaMemcpyAsync(&h->d_state.p->es_sigma2, h->pin.p->es, 2 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+    TRY(launch_estep(h, &h->d_state.p->es_sigma2, &h->d_state.p->es_w, h->d_ts.p));
     if (h->comm) {
-        TRY(allreduce(h, h->d_p1, (size_t)h->m));
-        TRY(allreduce(h, h->d_pxc, (size_t)h->m * 3));
+        TRY(allreduce(h, h->d_p1.p, (size_t)h->m));
+        TRY(allreduce(h, h->d_pxc.p, (size_t)h->m * 3));
     }
     return cpd_last_estep(h, pt1, p1, px, n_p);
 }
@@ -970,23 +988,20 @@ namespace {
 int bcpd_weights(cpd_ctx* h, const double* alpha, const double* sdiag, const int* perm, const double* ssw) {
     const long long m = h->m;
     const unsigned nb = blocks_for(m);
-    bcpd_la_kernel<<<nb, THREADS, 0, h->stream>>>(alpha, sdiag, m, ssw, h->dim, h->d_la64, h->d_la_part);
-    bcpd_la_finish_kernel<<<1, 32, 0, h->stream>>>(h->d_la_part, (int)nb, ssw, h->dim, h->n_global, h->d_log2c);
-    bcpd_la_apply_kernel<<<nb, THREADS, 0, h->stream>>>(h->d_la64, perm, m, h->d_log2c, h->d_la);
+    bcpd_la_kernel<<<nb, THREADS, 0, h->stream>>>(alpha, sdiag, m, ssw, h->dim, h->d_la64.p, h->d_la_part.p);
+    bcpd_la_finish_kernel<<<1, 32, 0, h->stream>>>(h->d_la_part.p, (int)nb, ssw, h->dim, h->n_global, h->d_log2c.p);
+    bcpd_la_apply_kernel<<<nb, THREADS, 0, h->stream>>>(h->d_la64.p, perm, m, h->d_log2c.p, h->d_la.p);
     KCHECK();
     h->launches += 3;
     return CPD_OK;
 }
 int ensure_weight_buffers(cpd_ctx* h) {
     const long long m = h->m;
-    if (h->la_cap < (size_t)m) {
-        TRY(dev_alloc(&h->d_la, (size_t)m));
-        TRY(dev_alloc(&h->d_la64, (size_t)m));
-        TRY(dev_alloc(&h->d_la_part, (size_t)blocks_for(m)));
-        h->la_cap = (size_t)m;
-    }
-    if (!h->d_log2c) TRY(dev_alloc(&h->d_log2c, 3));
-    if (!h->d_bc_es) TRY(dev_alloc(&h->d_bc_es, 3));
+    TRY(h->d_la.reserve((size_t)m));
+    TRY(h->d_la64.reserve((size_t)m));
+    TRY(h->d_la_part.reserve((size_t)blocks_for(m)));
+    if (!h->d_log2c.p) TRY(h->d_log2c.alloc(3));
+    if (!h->d_bc_es.p) TRY(h->d_bc_es.alloc(3));
     return CPD_OK;
 }
 }  // namespace
@@ -1017,29 +1032,29 @@ extern "C" int cpd_bcpd_estep(cpd_ctx* h, const double* t_source, double scale, 
     if (!any_weight) return fail(CPD_ERR_ARG, "every source has zero weight");
     TRY(ensure_weight_buffers(h));
     // alpha and sigma_diag (caller's order) into d_outM [0, m) and [m, 2m), {scale, sigma2, w} into d_bc_es
-    h->h_pin[44] = scale;
-    h->h_pin[45] = sigma2;
-    h->h_pin[46] = w;
-    CU(cudaMemcpyAsync(h->d_bc_es, h->h_pin + 44, 3 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-    CU(cudaMemcpyAsync(h->d_outM, alpha, (size_t)m * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-    CU(cudaMemcpyAsync(h->d_outM + m, sigma_diag, (size_t)m * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-    TRY(bcpd_weights(h, h->d_outM, h->d_outM + m, h->d_perm_src, h->d_bc_es));
-    if (h->raw_cap < (size_t)m * 3) { TRY(dev_alloc(&h->d_raw, (size_t)m * 3)); h->raw_cap = (size_t)m * 3; }
-    TRY(upload_cloud(h, t_source, m, h->d_raw));
-    gather3_kernel<<<blocks_for(m), THREADS, 0, h->stream>>>(h->d_raw, h->d_perm_src, m, 0.0, 0.0, 0.0, h->d_ts);
+    h->pin.p->bc_ssw[0] = scale;
+    h->pin.p->bc_ssw[1] = sigma2;
+    h->pin.p->bc_ssw[2] = w;
+    CU(cudaMemcpyAsync(h->d_bc_es.p, h->pin.p->bc_ssw, 3 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+    CU(cudaMemcpyAsync(h->d_outM.p, alpha, (size_t)m * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+    CU(cudaMemcpyAsync(h->d_outM.p + m, sigma_diag, (size_t)m * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+    TRY(bcpd_weights(h, h->d_outM.p, h->d_outM.p + m, h->d_perm_src.p, h->d_bc_es.p));
+    TRY(h->d_raw.reserve((size_t)m * 3));
+    TRY(upload_cloud(h, t_source, m, h->d_raw.p));
+    gather3_kernel<<<blocks_for(m), THREADS, 0, h->stream>>>(h->d_raw.p, h->d_perm_src.p, m, 0.0, 0.0, 0.0, h->d_ts.p);
     h->launches += 1;
     TRY(ensure_stats(h));
     h->cull_active = h->extent > 0.0 && 13.3 * sqrt(sigma2) < 0.25 * h->extent;
-    h->h_pin[32] = sigma2;
-    h->h_pin[33] = w;
-    CU(cudaMemcpyAsync(&h->d_state->es_sigma2, h->h_pin + 32, 2 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+    h->pin.p->es[0] = sigma2;
+    h->pin.p->es[1] = w;
+    CU(cudaMemcpyAsync(&h->d_state.p->es_sigma2, h->pin.p->es, 2 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
     h->wgt_on = true;
-    const int r = launch_estep(h, &h->d_state->es_sigma2, &h->d_state->es_w, h->d_ts);
+    const int r = launch_estep(h, &h->d_state.p->es_sigma2, &h->d_state.p->es_w, h->d_ts.p);
     h->wgt_on = false;
     TRY(r);
     if (h->comm) {
-        TRY(allreduce(h, h->d_p1, (size_t)m));
-        TRY(allreduce(h, h->d_pxc, (size_t)m * 3));
+        TRY(allreduce(h, h->d_p1.p, (size_t)m));
+        TRY(allreduce(h, h->d_pxc.p, (size_t)m * 3));
     }
     return cpd_last_estep(h, nu_d, nu, px, n_p);
 }
@@ -1049,35 +1064,35 @@ extern "C" int cpd_last_estep(cpd_ctx* h, double* pt1, double* p1, double* px, d
     if (!h->prepared) return fail(CPD_ERR_STATE, "no E-step has run on this handle");
     CU(cudaSetDevice(h->device));
     if (pt1) {
-        scatter_kernel<<<blocks_for(h->n), THREADS, 0, h->stream>>>(h->d_pt1, h->d_perm_tgt, h->n, 1, h->d_outN);
-        CU(cudaMemcpyAsync(pt1, h->d_outN, (size_t)h->n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+        scatter_kernel<<<blocks_for(h->n), THREADS, 0, h->stream>>>(h->d_pt1.p, h->d_perm_tgt.p, h->n, 1, h->d_outN.p);
+        CU(cudaMemcpyAsync(pt1, h->d_outN.p, (size_t)h->n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
         h->launches += 1;
     }
     if (p1) {
-        scatter_kernel<<<blocks_for(h->m), THREADS, 0, h->stream>>>(h->d_p1, h->d_perm_src, h->m, 1, h->d_outM);
-        CU(cudaMemcpyAsync(p1, h->d_outM, (size_t)h->m * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+        scatter_kernel<<<blocks_for(h->m), THREADS, 0, h->stream>>>(h->d_p1.p, h->d_perm_src.p, h->m, 1, h->d_outM.p);
+        CU(cudaMemcpyAsync(p1, h->d_outM.p, (size_t)h->m * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
         CU(cudaStreamSynchronize(h->stream));      // d_outM is reused for px below
         h->launches += 1;
     }
     if (px) {
-        uncentre_px_kernel<<<blocks_for(h->m), THREADS, 0, h->stream>>>(h->d_state, h->d_p1, h->d_pxc, (int)h->m, h->d_px);
-        scatter_kernel<<<blocks_for(h->m), THREADS, 0, h->stream>>>(h->d_px, h->d_perm_src, h->m, 3, h->d_outM);
+        uncentre_px_kernel<<<blocks_for(h->m), THREADS, 0, h->stream>>>(h->d_state.p, h->d_p1.p, h->d_pxc.p, (int)h->m, h->d_px.p);
+        scatter_kernel<<<blocks_for(h->m), THREADS, 0, h->stream>>>(h->d_px.p, h->d_perm_src.p, h->m, 3, h->d_outM.p);
         KCHECK();
         h->launches += 2;
-        TRY(download_cloud(h, h->d_outM, h->m, px));
+        TRY(download_cloud(h, h->d_outM.p, h->m, px));
     }
     if (n_p) {
         // n_p = sum(p1) (cpd.py:88): block partials of the (possibly all-reduced) p1
         const unsigned nb = blocks_for(h->m);
-        if (h->sums_cap < (size_t)nb * 4 + 4) { TRY(dev_alloc(&h->d_sums, (size_t)nb * 4 + 4)); h->sums_cap = (size_t)nb * 4 + 4; }
-        src_moments_api_kernel<<<nb, THREADS, 0, h->stream>>>((int)h->m, h->d_yc, h->d_p1, h->d_pxc, h->d_mom_src);
-        reduce_cols_kernel<<<1, MOM_SRC * 32, 0, h->stream>>>(h->d_mom_src, (int)nb, MOM_SRC, h->d_mom);
+        TRY(h->d_sums.reserve((size_t)nb * 4 + 4));
+        src_moments_api_kernel<<<nb, THREADS, 0, h->stream>>>((int)h->m, h->d_yc.p, h->d_p1.p, h->d_pxc.p, h->d_mom_src.p);
+        reduce_cols_kernel<<<1, MOM_SRC * 32, 0, h->stream>>>(h->d_mom_src.p, (int)nb, MOM_SRC, h->d_mom.p);
         KCHECK();
         h->launches += 2;
-        CU(cudaMemcpyAsync(h->h_pin + 40, h->d_mom, sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+        CU(cudaMemcpyAsync(&h->pin.p->n_p, h->d_mom.p, sizeof(double), cudaMemcpyDeviceToHost, h->stream));
     }
     CU(cudaStreamSynchronize(h->stream));
-    if (n_p) *n_p = h->h_pin[40];
+    if (n_p) *n_p = h->pin.p->n_p;
     return CPD_OK;
 }
 
@@ -1092,24 +1107,24 @@ extern "C" int cpd_mstep(cpd_ctx* h, int tf_kind, int update_scale, const double
     h->h_state.tf_kind = tf_kind;
     h->h_state.update_scale = update_scale ? 1 : 0;
     // only the two selectors: the rest of the device state may be ahead of the host mirror
-    CU(cudaMemcpyAsync(&h->d_state->tf_kind, &h->h_state.tf_kind, 2 * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    CU(cudaMemcpyAsync(&h->d_state.p->tf_kind, &h->h_state.tf_kind, 2 * sizeof(int), cudaMemcpyHostToDevice, h->stream));
     // caller's order -> internal (Morton) order
-    CU(cudaMemcpyAsync(h->d_outN, pt1, (size_t)h->n * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-    gather1_kernel<<<blocks_for(h->n), THREADS, 0, h->stream>>>(h->d_outN, h->d_perm_tgt, h->n, h->d_pt1);
-    CU(cudaMemcpyAsync(h->d_outM, p1, (size_t)h->m * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-    gather1_kernel<<<blocks_for(h->m), THREADS, 0, h->stream>>>(h->d_outM, h->d_perm_src, h->m, h->d_p1);
-    if (h->raw_cap < (size_t)h->m * 3) { TRY(dev_alloc(&h->d_raw, (size_t)h->m * 3)); h->raw_cap = (size_t)h->m * 3; }
-    TRY(upload_cloud(h, px, h->m, h->d_raw));
-    gather3_kernel<<<blocks_for(h->m), THREADS, 0, h->stream>>>(h->d_raw, h->d_perm_src, h->m, 0.0, 0.0, 0.0, h->d_px);
+    CU(cudaMemcpyAsync(h->d_outN.p, pt1, (size_t)h->n * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+    gather1_kernel<<<blocks_for(h->n), THREADS, 0, h->stream>>>(h->d_outN.p, h->d_perm_tgt.p, h->n, h->d_pt1.p);
+    CU(cudaMemcpyAsync(h->d_outM.p, p1, (size_t)h->m * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+    gather1_kernel<<<blocks_for(h->m), THREADS, 0, h->stream>>>(h->d_outM.p, h->d_perm_src.p, h->m, h->d_p1.p);
+    TRY(h->d_raw.reserve((size_t)h->m * 3));
+    TRY(upload_cloud(h, px, h->m, h->d_raw.p));
+    gather3_kernel<<<blocks_for(h->m), THREADS, 0, h->stream>>>(h->d_raw.p, h->d_perm_src.p, h->m, 0.0, 0.0, 0.0, h->d_px.p);
     h->launches += 3;
     const int nbs = (int)blocks_for(h->m), nbt = (int)blocks_for(h->n);
-    centre_px_kernel<<<nbs, THREADS, 0, h->stream>>>(h->d_state, h->d_p1, h->d_px, (int)h->m, h->d_pxc);
-    src_moments_api_kernel<<<nbs, THREADS, 0, h->stream>>>((int)h->m, h->d_yc, h->d_p1, h->d_pxc, h->d_mom_src);
-    tgt_moments_api_kernel<<<nbt, THREADS, 0, h->stream>>>(h->d_pt1, h->d_xc, (int)h->n, h->d_mom_tgt);
-    moments_kernel<0><<<1, 256, 0, h->stream>>>(h->d_state, h->d_mom_src, nbs, MOM_SRC, h->d_mom_tgt, nbt, MOM_TGT, h->d_mom);
+    centre_px_kernel<<<nbs, THREADS, 0, h->stream>>>(h->d_state.p, h->d_p1.p, h->d_px.p, (int)h->m, h->d_pxc.p);
+    src_moments_api_kernel<<<nbs, THREADS, 0, h->stream>>>((int)h->m, h->d_yc.p, h->d_p1.p, h->d_pxc.p, h->d_mom_src.p);
+    tgt_moments_api_kernel<<<nbt, THREADS, 0, h->stream>>>(h->d_pt1.p, h->d_xc.p, (int)h->n, h->d_mom_tgt.p);
+    moments_kernel<0><<<1, 256, 0, h->stream>>>(h->d_state.p, h->d_mom_src.p, nbs, MOM_SRC, h->d_mom_tgt.p, nbt, MOM_TGT, h->d_mom.p);
     KCHECK();
-    if (h->comm) TRY(allreduce(h, h->d_mom + MOM_SRC, MOM_TGT));   // p1/px are already global; pt1 is per shard
-    mstep_api_kernel<<<1, 32, 0, h->stream>>>(h->d_state, h->d_mom);
+    if (h->comm) TRY(allreduce(h, h->d_mom.p + MOM_SRC, MOM_TGT));   // p1/px are already global; pt1 is per shard
+    mstep_api_kernel<<<1, 32, 0, h->stream>>>(h->d_state.p, h->d_mom.p);
     KCHECK();
     h->launches += 5;
     return read_params(h, out);
