@@ -294,6 +294,23 @@ int cpd_filterreg_step(cpd_fr* h, const double* rot, const double* t, double sig
 int cpd_filterreg_get(cpd_fr* h, float* m0, float* m1, float* m2, float* nx, int* with_blur, int64_t* device_bytes, float* stage_ms);
 void cpd_filterreg_end(cpd_fr* h);
 
+/* Many independent rigid / affine registrations in one call, without a handle (no reference counterpart: the reference registers
+ * one pair at a time).  Pair k is source rows [src_off[k], src_off[k+1]) of src and target rows [tgt_off[k], tgt_off[k+1]) of tgt
+ * (both row-major, D = dim; src_off[0] = tgt_off[0] = 0; npairs + 1 offsets each).  Per pair exactly what cpd_sigma2_init +
+ * cpd_set_state + cpd_em_run(maxiter, tol) compute for it: sigma2_0 in closed form, q_0 = 1 + N D / 2 log sigma2_0 (cpd.py:148),
+ * then at most maxiter EM iterations, stopping after the first one with |q - q_prev| < tol.  init (NULL: identity, t = 0,
+ * scale = 1) holds npairs starting transformations (lin = rot or b, t, scale; scale is ignored for affine); sigma2 and q of init
+ * are not read.  out (npairs): the last MstepResult of each pair (the start state when maxiter = 0); iters (npairs): the
+ * iterations each pair ran.  One CTA owns one pair for its whole registration (csrc/batch.cuh): one launch and one read-back for
+ * the batch, and a pair's result does not depend on the other pairs, its position or the batch size.
+ * Refused with CPD_ERR_ARG before anything runs, naming the pair: an empty cloud, a non-finite coordinate or initial transformation,
+ * sigma2_0 = 0 (all points of both clouds identical), m or n > 2^16 or m n > 2^26 (such a pair belongs to the handle's
+ * loop); and dim not 2 or 3,
+ * w outside [0, 1), maxiter < 0, tf_kind not rigid or affine (CPD_TF_NONRIGID has its own message).                             */
+int cpd_batch_register(int device, int dim, int npairs, const double* src, const int64_t* src_off, const double* tgt,
+                       const int64_t* tgt_off, int tf_kind, int update_scale, double w, int maxiter, double tol,
+                       const cpd_params* init, cpd_params* out, int* iters);
+
 /* -- multi-GPU: one process per GPU, targets sharded, sources replicated -------------------
  * cpd_comm_unique_id fills 128 bytes (an ncclUniqueId) on one rank; after it has been
  * distributed (any side channel), every rank calls cpd_comm_create ONCE -- a collective -- and

@@ -90,6 +90,9 @@ _PROTOS = {
     "cpd_filterreg_get": (ctypes.c_int, [ctypes.c_void_p, _c_fp, _c_fp, _c_fp, _c_fp, ctypes.POINTER(ctypes.c_int),
                                          ctypes.POINTER(ctypes.c_int64), _c_fp]),
     "cpd_filterreg_end": (None, [ctypes.c_void_p]),
+    "cpd_batch_register": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_int, _c_dp, ctypes.POINTER(ctypes.c_int64), _c_dp,
+                                          ctypes.POINTER(ctypes.c_int64), ctypes.c_int, ctypes.c_int, ctypes.c_double, ctypes.c_int,
+                                          ctypes.c_double, ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(ctypes.c_int)]),
     "cpd_squared_kernel_sum": (ctypes.c_int, [ctypes.c_int, _c_dp, ctypes.c_int64, _c_dp, ctypes.c_int64, ctypes.c_int, _c_dp]),
     "cpd_comm_unique_id": (ctypes.c_int, [ctypes.c_char_p]),
     "cpd_comm_create": (ctypes.c_int, [ctypes.POINTER(ctypes.c_void_p), ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_char_p]),
@@ -575,6 +578,41 @@ def ocsvm_fit(x, nu, gamma, tol=1e-3, max_iter=None, device=0):
     check(lib().cpd_ocsvm_fit(device, dptr(xa), n, xa.shape[1], float(nu), float(gamma), float(tol), max_iter, dptr(alpha),
                               ctypes.byref(rho), ctypes.byref(it)))
     return alpha, rho.value, it.value
+
+
+def batch_register(src, src_off, tgt, tgt_off, dim, tf_kind, update_scale, w, maxiter, tol, init=None, device=0):
+    """Many rigid / affine registrations in one call (cpd_batch_register).  src, tgt: the concatenated clouds (rows x dim);
+    src_off, tgt_off: the B + 1 row offsets of the pairs; init: None or B (lin (dim x dim), t (dim), scale) tuples.
+    Returns a list of B (lin, t, scale, sigma2, q, n_p) tuples and the iterations each pair ran (int array)."""
+    s, t = as_cloud(src, dim), as_cloud(tgt, dim)
+    so = np.ascontiguousarray(src_off, dtype=np.int64)
+    to = np.ascontiguousarray(tgt_off, dtype=np.int64)
+    b = so.shape[0] - 1
+    if b < 1 or to.shape != so.shape:
+        raise ValueError("src_off and tgt_off must both hold B + 1 >= 2 offsets, got %s and %s" % (so.shape, to.shape))
+    ini = None
+    if init is not None:
+        ini = (CpdParams * b)()
+        for k, (lin, tt, scale) in enumerate(init):
+            lin = np.asarray(lin, dtype=np.float64).reshape(dim, dim)
+            tt = np.asarray(tt, dtype=np.float64).reshape(dim)
+            for i in range(dim):
+                ini[k].t[i] = tt[i]
+                for j in range(dim):
+                    ini[k].lin[i * dim + j] = lin[i, j]
+            ini[k].scale = float(scale)
+    out = (CpdParams * b)()
+    iters = np.zeros(b, dtype=np.int32)
+    check(lib().cpd_batch_register(int(device), int(dim), b, dptr(s), so.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)), dptr(t),
+                                   to.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)), int(tf_kind), int(bool(update_scale)), float(w),
+                                   int(maxiter), float(tol), ctypes.cast(ini, ctypes.c_void_p) if ini is not None else None,
+                                   ctypes.cast(out, ctypes.c_void_p), iters.ctypes.data_as(ctypes.POINTER(ctypes.c_int))))
+    res = []
+    for k in range(b):
+        p = out[k]
+        res.append((np.array(p.lin[: dim * dim], dtype=np.float64).reshape(dim, dim), np.array(p.t[:dim], dtype=np.float64), p.scale,
+                    p.sigma2, p.q, p.n_p))
+    return res, iters
 
 
 def fptr(a):

@@ -502,3 +502,72 @@ def registration_cpd(source, target, tf_type_name="rigid", w=0.0, maxiter=50, to
         raise ValueError("Unknown transformation type %s" % tf_type_name)
     cpd.set_callbacks(list(callbacks))
     return cpd.registration(_points(target), w, maxiter, tol)
+
+
+def registration_cpd_batch(sources, targets, tf_type_name="rigid", w=0.0, maxiter=50, tol=0.001, update_scale=True,
+                           tf_init_params=None, device=0):
+    """Many independent rigid or affine CPD registrations in one call (no reference counterpart: probreg registers one pair
+    per ``registration_cpd`` call).
+
+    sources, targets -- sequences of B arrays (or open3d point clouds); pair k is (sources[k], targets[k]).  Sizes may differ
+                        from pair to pair; every pair has the same D, 2 or 3
+    tf_type_name     -- 'rigid' | 'affine' ('nonrigid' and anything else: ValueError)
+    w, maxiter, tol  -- as in registration_cpd, for every pair
+    update_scale     -- RigidCPD's update_scale (rigid only)
+    tf_init_params   -- None, or B dicts with the keys registration_cpd takes (rigid: rot / t / scale, affine: b / t); an
+                        empty dict or None entry starts that pair from the identity
+    device           -- CUDA ordinal
+
+    Each pair gets exactly what ``registration_cpd(source, target, tf_type_name, w, maxiter, tol, update_scale=...,
+    tf_init_params=...)`` computes for it without callbacks: sigma2 from the closed form of ``cpd_sigma2_init``, q from
+    1 + N D / 2 log sigma2 (probreg/cpd.py:148) and the stop rule |q - q_prev| < tol after an iteration.  Callbacks are not
+    offered: the whole batch runs on the device (one CTA per pair, csrc/batch.cuh) with one read-back at the end.  A pair of
+    more than 2^16 points in a cloud or 2^26 point pairs (m n) is refused; it belongs to ``registration_cpd``.
+
+    Returns (results, n_iter): a list of B MstepResult (RigidTransformation / AffineTransformation, sigma2, q) and an int array
+    of the iterations each pair ran.
+    """
+    if tf_type_name in ("nonrigid", "nonrigid_constrained"):
+        raise ValueError("registration_cpd_batch registers rigid and affine pairs only; use registration_cpd for %s" % tf_type_name)
+    if tf_type_name not in ("rigid", "affine"):
+        raise ValueError("Unknown transformation type %s" % tf_type_name)
+    sources, targets = list(sources), list(targets)
+    if len(sources) != len(targets):
+        raise ValueError("sources and targets must have the same length, got %d and %d" % (len(sources), len(targets)))
+    b = len(sources)
+    if b == 0:
+        return [], np.zeros(0, dtype=np.int32)
+    srcs = [np.asarray(_points(s), dtype=np.float64) for s in sources]
+    tgts = [np.asarray(_points(t), dtype=np.float64) for t in targets]
+    dim = srcs[0].shape[1] if srcs[0].ndim == 2 else None
+    for k in range(b):
+        for name, a in (("source", srcs[k]), ("target", tgts[k])):
+            if a.ndim != 2 or a.shape[1] != dim:
+                raise ValueError("pair %d: the %s has shape %s; every cloud of the batch must be (count, %s)" % (k, name, a.shape, dim))
+    if dim not in (2, 3):
+        raise ValueError("probreg_b200 supports 2-D and 3-D points, got %s-D" % dim)
+    rigid = tf_type_name == "rigid"
+    init = None
+    if tf_init_params is not None:
+        tf_init_params = list(tf_init_params)
+        if len(tf_init_params) != b:
+            raise ValueError("tf_init_params must hold one dict per pair: %d for %d pairs" % (len(tf_init_params), b))
+        init = []
+        keys = {"rot", "t", "scale"} if rigid else {"b", "t"}
+        for k, params in enumerate(tf_init_params):
+            params = dict(params or {})
+            params.pop("xp", None)
+            bad = set(params) - keys
+            if bad:
+                raise ValueError("pair %d: unknown tf_init_params key(s) %s for %s CPD" % (k, sorted(bad), tf_type_name))
+            lin = params.get("rot" if rigid else "b", np.identity(dim))
+            init.append((lin, params.get("t", np.zeros(dim)), params.get("scale", 1.0) if rigid else 1.0))
+    src_off = np.r_[0, np.cumsum([s.shape[0] for s in srcs])]
+    tgt_off = np.r_[0, np.cumsum([t.shape[0] for t in tgts])]
+    out, iters = _cabi.batch_register(np.concatenate(srcs), src_off, np.concatenate(tgts), tgt_off, dim,
+                                      _cabi.TF_RIGID if rigid else _cabi.TF_AFFINE, update_scale, w, maxiter, tol, init, device)
+    results = []
+    for lin, t, scale, sigma2, q, _ in out:
+        tf_obj = tf.RigidTransformation(lin, t, scale, xp=np) if rigid else tf.AffineTransformation(lin, t)
+        results.append(MstepResult(tf_obj, sigma2, q))
+    return results, iters

@@ -10,6 +10,7 @@
 #include "l2dist.cuh"
 #include "ocsvm.cuh"
 #include "lattice.cuh"
+#include "batch.cuh"
 
 #include <cub/device/device_radix_sort.cuh>
 #ifdef CPD_HOST_EMU
@@ -834,14 +835,7 @@ extern "C" int cpd_sigma2_init(cpd_ctx* h, double* sigma2) {
     CU(cudaStreamSynchronize(h->stream));
     TRY(ensure_stats(h));
     for (int k = 0; k < 4; ++k) { sx[k] = h->pin.p->sums[k]; sy[k] = h->pin.p->sums[4 + k]; }
-    // move the source sums into the targets' frame: y' = y~ + (cy - cx)
-    double dlt[3], d2 = 0.0, dsy = 0.0;
-    for (int a = 0; a < 3; ++a) { dlt[a] = h->h_state.cy[a] - h->h_state.cx[a]; d2 += dlt[a] * dlt[a]; dsy += dlt[a] * sy[1 + a]; }
-    const double M = (double)h->m, N = (double)h->n_global;
-    const double syy = sy[0] + 2.0 * dsy + M * d2;
-    double cross = 0.0;
-    for (int a = 0; a < 3; ++a) cross += sx[1 + a] * (sy[1 + a] + M * dlt[a]);
-    *sigma2 = (M * sx[0] + N * syy - 2.0 * cross) / (M * N * h->dim);
+    *sigma2 = sigma2_closed_form(sx, sy, h->h_state.cx, h->h_state.cy, (double)h->m, (double)h->n_global, h->dim);
     return CPD_OK;
 }
 
@@ -1130,7 +1124,7 @@ extern "C" int cpd_mstep(cpd_ctx* h, int tf_kind, int update_scale, const double
     return read_params(h, out);
 }
 
-// The remaining entry points live in six .inl files of this same translation unit:
+// The remaining entry points live in the .inl files of this same translation unit:
 #include "host_nonrigid.inl"     // cpd_nonrigid_* (dense G, low-rank factors, priors)
 #include "host_bcpd.inl"         // cpd_bcpd_begin / step / get, cpd_bcpd_step_times (the BCPD loop on the device)
 #include "host_gmmtree.inl"      // cpd_gmmtree_* (the GMMTree build and registration E-step)
@@ -1140,3 +1134,4 @@ extern "C" int cpd_mstep(cpd_ctx* h, int tf_kind, int update_scale, const double
 #include "host_filterreg.inl"    // cpd_lattice_filter, cpd_filterreg_estep (the permutohedral lattice of FilterReg)
 #include "host_multi.inl"        // cpd_comm_*, cpd_p2p_*
 #include "host_measure.inl"      // cpd_timer_*, cpd_event_*, cpd_stage_times, cpd_flush_l2, cpd_microbench
+#include "host_batch.inl"        // cpd_batch_register (many small rigid / affine registrations, one CTA per pair)

@@ -245,6 +245,35 @@ __device__ __forceinline__ void block_reduce_store(double (&v)[K], double* out) 
     }
 }
 
+// The current transform in the targets' frame, on the centred sources: z~ = l y~ + tp with l = scale R (rigid) or B (affine) and
+// tp = l cy + t - cx.  One FP64 evaluation (pack_kernel, batch_em_kernel).
+__device__ __forceinline__ void frame_transform(const DevState& st, double (&l)[9], double (&tp)[3]) {
+    const double s = (st.tf_kind == 0) ? st.scale : 1.0;
+#pragma unroll
+    for (int k = 0; k < 9; ++k) l[k] = s * st.lin[k];
+#pragma unroll
+    for (int a = 0; a < 3; ++a)
+        tp[a] = l[3 * a] * st.cy[0] + l[3 * a + 1] * st.cy[1] + l[3 * a + 2] * st.cy[2] + st.t[a] - st.cx[a];
+}
+__device__ __forceinline__ void frame_apply(const double (&l)[9], const double (&tp)[3], double y0, double y1, double y2, double& px,
+                                            double& py, double& pz) {
+    px = l[0] * y0 + l[1] * y1 + l[2] * y2 + tp[0];
+    py = l[3] * y0 + l[4] * y1 + l[5] * y2 + tp[1];
+    pz = l[6] * y0 + l[7] * y1 + l[8] * y2 + tp[2];
+}
+// sigma2_0 of math_utils.squared_kernel_sum in closed form (cpd_sigma2_init, batch_em_kernel): sx = {sum |x|^2, sum x} of the targets
+// centred on cx, sy = the same of the sources centred on cy, M sources, N targets, D = dim.
+__host__ __device__ inline double sigma2_closed_form(const double* sx, const double* sy, const double* cx, const double* cy, double M,
+                                                     double N, int dim) {
+    // move the source sums into the targets' frame: y' = y~ + (cy - cx)
+    double dlt[3], d2 = 0.0, dsy = 0.0;
+    for (int a = 0; a < 3; ++a) { dlt[a] = cy[a] - cx[a]; d2 += dlt[a] * dlt[a]; dsy += dlt[a] * sy[1 + a]; }
+    const double syy = sy[0] + 2.0 * dsy + M * d2;
+    double cross = 0.0;
+    for (int a = 0; a < 3; ++a) cross += sx[1 + a] * (sy[1 + a] + M * dlt[a]);
+    return (M * sx[0] + N * syy - 2.0 * cross) / (M * N * dim);
+}
+
 // ---------------------------------------------------------------------------------------------
 // pack: transform + centre + scale both clouds into the FP32 working frame
 //   a_m = sk * (lin_eff * (y_m - cy) + t')   with t' = lin_eff*cy + t - cx     (sources)
@@ -270,17 +299,9 @@ pack_kernel(const DevState* __restrict__ st, const double* __restrict__ sigma2_p
                 py = ts[3 * i + 1] - st->cx[1];
                 pz = ts[3 * i + 2] - st->cx[2];
             } else {
-                const double s = (st->tf_kind == 0) ? st->scale : 1.0;
                 double l[9], tp[3];
-#pragma unroll
-                for (int k = 0; k < 9; ++k) l[k] = s * st->lin[k];
-#pragma unroll
-                for (int a = 0; a < 3; ++a)
-                    tp[a] = l[3 * a] * st->cy[0] + l[3 * a + 1] * st->cy[1] + l[3 * a + 2] * st->cy[2] + st->t[a] - st->cx[a];
-                const double y0 = yc[3 * i], y1 = yc[3 * i + 1], y2 = yc[3 * i + 2];
-                px = l[0] * y0 + l[1] * y1 + l[2] * y2 + tp[0];
-                py = l[3] * y0 + l[4] * y1 + l[5] * y2 + tp[1];
-                pz = l[6] * y0 + l[7] * y1 + l[8] * y2 + tp[2];
+                frame_transform(*st, l, tp);
+                frame_apply(l, tp, yc[3 * i], yc[3 * i + 1], yc[3 * i + 2], px, py, pz);
             }
             o = make_float4((float)(sk * px), (float)(sk * py), (float)(sk * pz), 0.0f);
         } else {
@@ -671,6 +692,42 @@ pass1_kernel(const float4* __restrict__ ipts, int ni, const float4* __restrict__
 //            dead / padding: -omin = +inf (so 2^-(u - omin) == 0), rn = 0
 // and the target-side moments: Srr = sum_n SU_n rn_n (= sum_mn P_mn u_mn), Npt = sum pt1.
 // ---------------------------------------------------------------------------------------------
+// c = (2 pi sigma2)^(D/2) w/(1-w) M/N of cpd.py:78-79 (0 when w == 0)
+__device__ __forceinline__ double outlier_constant(double sigma2, double w, int dim, long long m, long long n_global) {
+    double c = 0.0;
+    if (w > 0.0) {
+        const double tps = 2.0 * 3.14159265358979323846 * sigma2;
+        c = (dim == 3 ? tps * sqrt(tps) : tps) * (w / (1.0 - w) * (double)m / (double)n_global);
+    }
+    return c;
+}
+// The column arithmetic of finalize 1 (also batch.cuh's per-thread finalize): from log2 S (the column's log2 sum_m K), c (> 0: an
+// outlier constant with log2 lc), the dead-column shift and the column's integer offset omin with its SU, the column's pt1, the
+// pass-2 record's -omin (no; +inf when dead) and rn rounded once to FP32 (rnf; 0 when dead), and its Srr term SU rnf.
+__device__ __forceinline__ void finalize_column(double log2S, double c, double lc, double dead_shift, float omin, double SU, double& p1n,
+                                                float& no, float& rnf, double& srr) {
+    const bool dead = !(log2S + dead_shift >= DEAD_LOG2);
+    double L = 0.0;
+    p1n = 0.0;
+    if (!dead) {
+        if (c > 0.0) {
+            const double hi = fmax(log2S, lc), lo = fmin(log2S, lc);
+            L = hi + log2(1.0 + exp2(lo - hi));
+            p1n = exp2(log2S - L);
+        } else {
+            L = log2S; p1n = 1.0;
+        }
+    }
+    no = INFINITY;
+    rnf = 0.0f;
+    srr = 0.0;
+    if (!dead) {
+        const double rn = exp2(-(L + (double)omin));
+        no = -omin;
+        rnf = (float)rn;
+        srr = SU * (double)rnf;       // the same (rounded) rn that pass 2 multiplies by
+    }
+}
 __global__ void __launch_bounds__(THREADS)
 finalize1_kernel(const DevState* __restrict__ st, const double* __restrict__ sigma2_ptr, const double* __restrict__ w_ptr,
                  const P1Part* __restrict__ part, const int* __restrict__ tile_slots, int n, const float4* __restrict__ tgtP,
@@ -698,34 +755,15 @@ finalize1_kernel(const DevState* __restrict__ st, const double* __restrict__ sig
             }
             log2S = log2(S) - (double)omin;
         }
-        const double sigma2 = *sigma2_ptr, w = *w_ptr;
-        double c = 0.0;
-        if (w > 0.0) {
-            const double tps = 2.0 * 3.14159265358979323846 * sigma2;
-            c = (st->dim == 3 ? tps * sqrt(tps) : tps) * (w / (1.0 - w) * (double)st->m / (double)st->n_global);
-        }
+        double c = outlier_constant(*sigma2_ptr, *w_ptr, st->dim, st->m, st->n_global);
         double lc = c > 0.0 ? log2(c) : -INFINITY, dead_shift = 0.0;
         if (log2c_ptr != nullptr) { lc = log2c_ptr[0]; dead_shift = log2c_ptr[1]; c = (lc > -INFINITY) ? 1.0 : 0.0; }
-        const bool dead = !(log2S + dead_shift >= DEAD_LOG2);
-        double L = 0.0, p1n = 0.0;
-        if (!dead) {
-            if (c > 0.0) {
-                const double hi = fmax(log2S, lc), lo = fmin(log2S, lc);
-                L = hi + log2(1.0 + exp2(lo - hi));
-                p1n = exp2(log2S - L);
-            } else {
-                L = log2S; p1n = 1.0;
-            }
-        }
+        double p1n, srr;
+        float no, rnf;
+        finalize_column(log2S, c, lc, dead_shift, omin, SU, p1n, no, rnf, srr);
         pt1[i] = p1n;
         const float4 b = tgtP[i];
-        float no = INFINITY, rnf = 0.0f;
-        if (!dead) {
-            const double rn = exp2(-(L + (double)omin));
-            no = -omin;
-            rnf = (float)rn;
-            v[0] = SU * (double)rnf;       // the same (rounded) rn that pass 2 multiplies by
-        }
+        v[0] = srr;
         v[1] = p1n;
         tgtQ[2 * (size_t)i] = make_float4(b.x, b.y, b.z, no);
         tgtQ[2 * (size_t)i + 1] = make_float4(rnf, 0.f, 0.f, 0.f);
