@@ -69,7 +69,10 @@ int cpd_sigma2_init(cpd_ctx* h, double* sigma2);
 
 /* Set the state the EM loop starts from: family, RigidCPD(update_scale=...) (cpd.py:136),
  * the outlier weight w of registration() (cpd.py:106), tf_init_params (cpd.py:149-152:
- * lin = rot or b, t, scale) and sigma2 / q of _initialize (cpd.py:145-153).             */
+ * lin = rot or b, t, scale) and sigma2 / q of _initialize (cpd.py:145-153).
+ * The EM loop and the non-rigid loop share the device state: this call (and cpd_mstep)
+ * ends a non-rigid loop on the handle, and cpd_nonrigid_*begin / cpd_nonrigid_restart end
+ * this loop.  A later call on the ended loop fails with CPD_ERR_STATE, naming the call.  */
 int cpd_set_state(cpd_ctx* h, int tf_kind, int update_scale, double w, const cpd_params* init);
 
 /* One EM iteration == the loop body cpd.py:111-113: transform(source) -> expectation_step

@@ -143,7 +143,7 @@ int load_cusolver() {
     g_sol.lib = lib;
     return CPD_OK;
 }
-constexpr int CUDA_R_64F_ = 1, CUBLAS_OP_T_ = 1;
+constexpr int CUDA_R_64F_ = 1, CUBLAS_OP_N_ = 0, CUBLAS_OP_T_ = 1;
 }  // namespace
 #define SOLV(call)                                                                          \
     do {                                                                                    \
@@ -236,6 +236,115 @@ struct PinStage {
     double gt_q;             // cpd_gmmtree_build: the log-likelihood of an iteration
     double gt_rt[12];        // cpd_gmmtree_estep: rot (9) and t (3)
 };
+
+// cuSOLVER's dense LU (getrf: the column-major n x n matrix at `a` in place; getrs: op(A) X = B for the nrhs columns of `b`),
+// created on first use.  The workspace only grows: a loop that sized it for its system still finds enough after another loop
+// sized it for a smaller one.
+struct Solver {
+    void *h = nullptr, *params = nullptr;
+    DevBuf<unsigned char> d_work;
+    std::vector<unsigned char> h_work;
+    ~Solver() {
+        if (params && g_sol.DestroyParams) g_sol.DestroyParams(params);
+        if (h && g_sol.Destroy) g_sol.Destroy(h);
+    }
+    // after load_cusolver: the handle on `stream` and a workspace for the LU of the n x n system stored at `a`
+    int reserve(cudaStream_t stream, long long n, double* a) {
+        if (!h) {
+            SOLV(g_sol.Create(&h));
+            SOLV(g_sol.SetStream(h, stream));
+            SOLV(g_sol.CreateParams(&params));
+        }
+        size_t wd = 0, wh = 0;
+        SOLV(g_sol.XgetrfBuf(h, params, n, n, CUDA_R_64F_, a, n, CUDA_R_64F_, &wd, &wh));
+        TRY(d_work.reserve(std::max<size_t>(wd, 16)));
+        if (wh > h_work.size() || h_work.empty()) h_work.resize(std::max<size_t>(wh, 16));
+        return CPD_OK;
+    }
+    int getrf(long long n, double* a, int64_t* ipiv, int* info) {
+        SOLV(g_sol.Xgetrf(h, params, n, n, CUDA_R_64F_, a, n, ipiv, CUDA_R_64F_, d_work.p, d_work.n, h_work.data(), h_work.size(), info));
+        return CPD_OK;
+    }
+    int getrs(int op, long long n, long long nrhs, const double* a, const int64_t* ipiv, double* b, int* info) {
+        SOLV(g_sol.Xgetrs(h, params, op, n, nrhs, CUDA_R_64F_, a, n, ipiv, CUDA_R_64F_, b, n, info));
+        return CPD_OK;
+    }
+};
+
+// The loops a handle runs between calls keep what they need from one call to the next in records of their own.  The rigid / affine EM loop (cpd_set_state, cpd_em_step): DevState's transformation, shared with the non-rigid loop, which
+// ends it (and is ended by it)
+enum class EmStatus { none, live, ended };
+
+// whose set-up the low-rank factors hold, hence which kernel function the G X products use
+enum class LrOwner { none, nonrigid, bcpd };
+// G ~= Q Bc Q^T of rank `rank` (lowrank.cuh): the set-up of the low-rank non-rigid or BCPD loop, whichever began last
+struct LowRankFactors {
+    LrOwner owner = LrOwner::none;
+    int rank = 0;                         // > 0: a set-up finished
+    long long m = 0;                      // source count the buffers were sized for (the owner's at its begin)
+    double gscale = 1.0;                  // the factor of the products beyond the tile values: c^(-1/2) for the IMQ, 1 for the Gaussian
+    bool spd = true;                      // symmetric positive definite K x K system on Qt = Q L (lr_spd_form); CPD_B200_LR_CORE=lu: LU of (c I + Bc S)
+    float setup_ms[3] = {0.f, 0.f, 0.f};  // products / orthonormalisations / core of the last profiled set-up
+    DevBuf<float4> pts;
+    DevBuf<double> Q, X, coef, part, Bc, S, R, sys, rhs, c, out, panel, Lt;
+    DevBuf<int> pchol_rank;               // the rank lr_pchol_kernel found
+    DevBuf<unsigned char> gi_planes;      // exact int8-digit product: digit planes of X, FP64 chunk partials, column maxima
+    DevBuf<double> gi_part, gi_colmax;
+};
+
+// non-rigid CPD (host_nonrigid.inl): dense G, or the low-rank factors of LowRankFactors
+enum class NrStatus { none, dense, lowrank, ended };
+struct NonRigidLoop {
+    NrStatus status = NrStatus::none;
+    const char* ended_by = nullptr;       // status == ended: the refusal, which names the call that ended the loop
+    double lmd = 0.0;
+    bool w_stale = false;                 // low-rank: W is formed on demand (cpd_nonrigid_get) from B, wgt, ts and lr.c
+    bool prior_on = false;                // the correspondence priors of ConstrainedNonRigidCPD: alpha, p1t, pxt
+    double alpha = 1.0;
+    DevBuf<float> G;
+    DevBuf<double> W, A, B, part;
+    DevBuf<double> ts, ts2;               // the moved source T = Y + G W, and the next one while a step forms it (ts: 3 m, allocated last)
+    DevBuf<double> wgt;                   // the weights of the last solve: nr_weight_kernel's with priors, else a copy of p1 (low-rank)
+    DevBuf<int64_t> ipiv;
+    DevBuf<int> info;                     // cuSOLVER's info
+    DevBuf<double> p1t, pxt;
+    bool live() const { return status == NrStatus::dense || status == NrStatus::lowrank; }
+    void end(const char* why) { if (live()) { status = NrStatus::ended; ended_by = why; } }
+};
+
+// the BCPD registration loop (host_bcpd.inl): G^-1 (float32), the precision A and Sigma (FP64), all M x M in the internal order
+enum class BcStatus { none, running, stopped };   // stopped: a step failed (LU, sigma2); the loop needs a new begin
+struct BcpdLoop {
+    BcStatus status = BcStatus::none;
+    bool lowrank = false;                 // the K x K M-step on the factors of LowRankFactors (cpd_bcpd_lowrank_begin)
+    long long m = 0;                      // source count of the last begin
+    double sigma2 = 0.0;                  // host copy of the sigma2 the next E-step uses (culling decision)
+    DevBuf<BcpdState> state;
+    DevBuf<float> ginv;
+    DevBuf<double> A, S, v, r, alpha, sdiag, part, sums;
+    DevBuf<int64_t> ipiv;
+    DevBuf<int> info;                     // [0] getrf's info, [1] getrs's
+    // low-rank mode: the K x K system and C = its inverse, C Qt^T ([K][ld]), r in [3][m], w = C Rt (K x 3) and the pivots of the K x K LU
+    DevBuf<double> sys, C, CQ, rt, w;
+    DevBuf<int64_t> lr_ipiv;
+    Event ev[6];
+    float ms[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
+    // the dense loop's M x M buffers (and pivots), released before either begin allocates
+    void release_dense() { ginv.reset(); A.reset(); S.reset(); ipiv.reset(); }
+};
+
+// GMMTree (host_gmmtree.inl, gmmtree.cuh): the tree (13 doubles per node), its prepared form (16) and the per-point work arrays
+struct GmmTree {
+    int levels = 0;                       // > 0: a tree is installed (cpd_gmmtree_build / cpd_gmmtree_load)
+    long long total = 0, m = 0;           // nodes, source count of the last build (0: loaded)
+    DevBuf<double> nodes, prep, pts, spts, g, part, mom, scr;
+    DevBuf<unsigned> keys, keys2;
+    DevBuf<int> idx, idx2, cur, start, end, asg;
+    DevBuf<long long> seeds;
+    DevBuf<unsigned char> sort;
+    Event ev[7];
+    float ms[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};   // build ms per level (up to 5), ms of the last registration E-step
+};
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------
@@ -273,7 +382,9 @@ struct cpd_ctx {
     double extent = 0.0;              // largest bounding-box edge of the target shard (caller units)
     DevBuf<int4> d_work1, d_work2;
     DevBuf<int> d_slots1, d_slots2;
-    bool have_source = false, have_target = false, have_state = false, prepared = false;
+    bool have_source = false, have_target = false, prepared = false;
+    EmStatus em = EmStatus::none;
+    const char* em_ended_by = nullptr;    // em == ended: the call that ended the EM loop
     nccl_comm comm = nullptr;
     int world = 1, rank = 0;
     // Morton ordering (internal permutation; results leave in the caller's order)
@@ -281,70 +392,16 @@ struct cpd_ctx {
     DevBuf<unsigned> d_codes, d_codes_out;
     DevBuf<unsigned char> d_sort_tmp;
     DevBuf<double> d_outN, d_outM;      // staging for un-permuted outputs / permuted inputs
-    // non-rigid CPD (dense G)
-    DevBuf<float> d_G;
-    DevBuf<double> d_W, d_A, d_B, d_ts2, d_nrpart;
-    DevBuf<int64_t> d_ipiv;
-    DevBuf<int> d_info;
-    DevBuf<unsigned char> d_work;        // the solver's workspace, device and host
-    std::vector<unsigned char> h_work;
-    void *sol = nullptr, *sol_params = nullptr;
-    long long nr_m = 0;
-    double nr_lmd = 0.0;
-    bool nr_ready = false;
-    bool nr_lost_to_bcpd = false;         // the non-rigid loop ended because cpd_bcpd_lowrank_begin took the low-rank factors
     // weighted E-step (BCPD): per-source exponent offsets (FP64 scratch, block minima, the float32 values the passes read) and
     // {log2 c, dead-column shift, la_min} for finalize 1; d_bc_es: {scale, sigma2, w} of a stand-alone cpd_bcpd_estep
     DevBuf<float> d_la;
     DevBuf<double> d_la64, d_la_part, d_bc_es;
     DevBuf<double> d_log2c;
-    bool wgt_on = false;
-    // BCPD registration loop (host_bcpd.inl): G^-1 (float32), the precision A and Sigma (FP64), all M x M in the internal order
-    DevBuf<BcpdState> d_bc;
-    DevBuf<float> d_bc_ginv;
-    DevBuf<double> d_bc_A, d_bc_S, d_bc_v, d_bc_r, d_bc_alpha, d_bc_sdiag, d_bc_part, d_bc_sums;
-    DevBuf<int64_t> d_bc_ipiv;
-    DevBuf<int> d_bc_info;                // [0] getrf's info, [1] getrs's
-    long long bc_m = 0;                   // source count the buffers were sized for
-    double bc_sigma2 = 0.0;               // host copy of the sigma2 the next E-step uses (culling decision)
-    bool bc_ready = false;
-    bool bc_stopped = false;              // a step failed (LU, sigma2): the loop needs a new cpd_bcpd_begin
-    Event bc_ev[6];
-    float bc_ms[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
-    // low-rank mode (cpd_bcpd_lowrank_begin): the factor is the handle's low-rank Qt (d_lr_X); the K x K system and C = its
-    // inverse, C Qt^T ([K][ld]), r in [3][m], w = C Rt (K x 3) and the pivots of the K x K LU
-    bool bc_lowrank = false;
-    DevBuf<double> d_bc_sys, d_bc_C, d_bc_CQ, d_bc_rt, d_bc_w;
-    DevBuf<int64_t> d_bc_lr_ipiv;
-    // GMMTree (host_gmmtree.inl, gmmtree.cuh): the tree (13 doubles per node) and its prepared form (16), per-point work arrays
-    // (coordinates, sorted coordinates, 8 gammas, sort keys / values in and out, argmax), the run bounds of the keys, the chunk
-    // partials, the moments of a registration E-step and scratch
-    int gt_levels = 0;                    // > 0: a tree is installed (cpd_gmmtree_build / cpd_gmmtree_load)
-    long long gt_total = 0, gt_m = 0;     // nodes, source count of the last build (0: loaded)
-    DevBuf<double> d_gt_nodes, d_gt_prep, d_gt_pts, d_gt_spts, d_gt_g, d_gt_part, d_gt_mom, d_gt_scr;
-    DevBuf<unsigned> d_gt_keys, d_gt_keys2;
-    DevBuf<int> d_gt_idx, d_gt_idx2, d_gt_cur, d_gt_start, d_gt_end, d_gt_asg;
-    DevBuf<long long> d_gt_seeds;
-    DevBuf<unsigned char> d_gt_sort;
-    Event gt_ev[7];
-    float gt_ms[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};   // build ms per level (up to 5), ms of the last registration E-step
-    // correspondence priors of ConstrainedNonRigidCPD
-    DevBuf<double> d_wgt, d_p1t, d_pxt;
-    long long prior_m = 0;
-    double prior_alpha = 1.0;
-    bool prior_on = false;
-    // non-rigid CPD, rank-K G ~= Q Bc Q^T (lowrank.cuh)
-    int lr_rank = 0;                      // > 0: cpd_nonrigid_step takes the low-rank M-step
-    int lr_owner = 0;                     // whose set-up the factors are: LR_OWNER_NONE / _NONRIGID (Gaussian G) / _BCPD (IMQ G)
-    double lr_gscale = 1.0;               // the factor of the products beyond the tile values: c^(-1/2) for the IMQ, 1 for the Gaussian
-    bool lr_w_stale = false;              // W of the low-rank path is formed on demand
-    float lr_setup_ms[3] = {0.f, 0.f, 0.f};   // products / orthonormalisations / core of the last profiled set-up
-    long long lr_m = 0;
-    DevBuf<float4> d_lr_pts;
-    DevBuf<double> d_lr_Q, d_lr_X, d_lr_coef, d_lr_part, d_lr_Bc, d_lr_S, d_lr_R, d_lr_sys, d_lr_rhs, d_lr_c, d_lr_out, d_lr_panel, d_lr_Lt;
-    bool lr_spd = true;                   // symmetric positive definite K x K system on Qt = Q L (lr_spd_form); CPD_B200_LR_CORE=lu: LU of (c I + Bc S)
-    DevBuf<unsigned char> d_gi_planes;    // exact int8-digit product: digit planes of X, FP64 chunk partials, column maxima
-    DevBuf<double> d_gi_part, d_gi_colmax;
+    Solver sol;
+    LowRankFactors lr;
+    NonRigidLoop nr;
+    BcpdLoop bc;
+    GmmTree gt;
     DevBuf<P2PMailbox> d_box;             // this rank's mailbox (peers write into it)
     DevBuf<P2PInfo> d_p2p;                // device copy of the peer table; allocated => fused P2P exchange
     void* peer_ptr[P2P_MAX] = {nullptr};  // mappings opened with cudaIpcOpenMemHandle
@@ -483,6 +540,16 @@ int download_cloud(cpd_ctx* h, const double* src3, long long count, double* dst)
     }
     return CPD_OK;
 }
+// a per-source device array (cols 1 or 3, internal order) into the caller's order at `out`; returns once it has arrived
+int download_src(cpd_ctx* h, const double* d, int cols, double* out) {
+    scatter_kernel<<<blocks_for(h->m), THREADS, 0, h->stream>>>(d, h->d_perm_src.p, h->m, cols, h->d_outM.p);
+    KCHECK();
+    h->launches += 1;
+    if (cols == 3) TRY(download_cloud(h, h->d_outM.p, h->m, out));
+    else CU(cudaMemcpyAsync(out, h->d_outM.p, (size_t)h->m * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+    CU(cudaStreamSynchronize(h->stream));        // d_outM is reused
+    return CPD_OK;
+}
 
 // d_out[0] = sum |p|^2, d_out[1..3] = sum p   over a device count x 3 cloud; stays on the device (stream-ordered, no sync).
 // `part`: blocks_for(count) * 4 doubles of scratch.
@@ -548,10 +615,22 @@ int ensure_stats(cpd_ctx* h) {
     return CPD_OK;
 }
 
+int require_clouds(cpd_ctx* h) {
+    if (!h->have_source || !h->have_target) return fail(CPD_ERR_STATE, "source and target must both be set");
+    return CPD_OK;
+}
+
+// culling for an E-step at sigma2: a point reaches ~13.3 sigma (2^-127); culling can only pay once that is well inside the cloud
+int decide_cull(cpd_ctx* h, double sigma2) {
+    TRY(ensure_stats(h));
+    h->cull_active = h->extent > 0.0 && 13.3 * sqrt(sigma2) < 0.25 * h->extent;
+    return CPD_OK;
+}
+
 int prepare(cpd_ctx* h) {
     TRY(ensure_stats(h));
     if (h->prepared) return CPD_OK;
-    if (!h->have_source || !h->have_target) return fail(CPD_ERR_STATE, "source and target must both be set");
+    TRY(require_clouds(h));
     h->it1 = (int)((h->n + ITILE1 - 1) / ITILE1);
     h->it2 = (int)((h->m + ITILE2 - 1) / ITILE2);
     // Pass 1 cuts at sub-chunks, and the warps of its last i-tile whose i-points are all padding leave the kernel at once.  Such a
@@ -605,18 +684,20 @@ int allreduce(cpd_ctx* h, double* buf, size_t count) {
     return CPD_OK;
 }
 
-inline void mark(cpd_ctx* h, int k) {
-    if (h->profiling) cudaEventRecord(h->sev[k], h->stream);
+// a profiling event (cpd_set_profiling)
+inline void mark(cpd_ctx* h, cudaEvent_t e) {
+    if (h->profiling) cudaEventRecord(e, h->stream);
 }
 
-// pack + pass 1 + finalize 1 + pass 2 + finalize 2; sigma2/w read from the given device scalars
-int launch_estep(cpd_ctx* h, const double* d_sigma2, const double* d_w, const double* d_ts) {
+// pack + pass 1 + finalize 1 + pass 2 + finalize 2; sigma2/w read from the given device scalars; wgt: with the per-source
+// exponents of bcpd_weights (BCPD)
+int launch_estep(cpd_ctx* h, const double* d_sigma2, const double* d_w, const double* d_ts, bool wgt) {
     TRY(prepare(h));
     const long long cover = std::max(h->mpad, h->n);
-    mark(h, 0);
+    mark(h, h->sev[0]);
     pack_kernel<<<blocks_for(cover), THREADS, 0, h->stream>>>(h->d_state.p, d_sigma2, h->d_yc.p, d_ts, h->d_xc.p, h->m, h->mpad,
                                                               h->n, h->d_srcP.p, h->d_tgtP.p);
-    mark(h, 1);
+    mark(h, h->sev[1]);
     const bool cull = h->cull_on && h->cull_active;
     const int nst1 = (int)(h->mpad / P1_STAGE);
     stage_bbox_kernel<<<(unsigned)nst1, THREADS, 0, h->stream>>>(h->d_srcP.p, (int)h->m, P1_STAGE, h->d_sbox.p);   // offset seeding (always)
@@ -628,7 +709,6 @@ int launch_estep(cpd_ctx* h, const double* d_sigma2, const double* d_w, const do
         sub_bbox_kernel<<<(unsigned)((nsub2 + 7) / 8), THREADS, 0, h->stream>>>(h->d_tgtP.p, (int)h->n, nsub2, h->d_tsub.p);
         h->launches += 3;
     }
-    const bool wgt = h->wgt_on;
     if (wgt) {
         weight_patch_kernel<<<blocks_for(h->m), THREADS, 0, h->stream>>>(h->d_la.p, h->m, h->d_srcP.p);
         h->launches += 1;
@@ -637,11 +717,11 @@ int launch_estep(cpd_ctx* h, const double* d_sigma2, const double* d_w, const do
     if (cull) { if (wgt) CPD_PASS1(true, true); else CPD_PASS1(true, false); }
     else { if (wgt) CPD_PASS1(false, true); else CPD_PASS1(false, false); }
 #undef CPD_PASS1
-    mark(h, 2);
+    mark(h, h->sev[2]);
     finalize1_kernel<<<blocks_for(h->npad), THREADS, 0, h->stream>>>(h->d_state.p, d_sigma2, d_w, h->d_part1.p, h->d_slots1.p, (int)h->n,
                                                                      h->d_tgtP.p, h->d_tgtQ.p, h->npad, h->d_pt1.p, h->d_mom_tgt.p,
                                                                      wgt ? h->d_log2c.p : nullptr);
-    mark(h, 3);
+    mark(h, h->sev[3]);
     if (cull) {
         stage_omax_kernel<<<(unsigned)(h->npad / P2_STAGE), THREADS, 0, h->stream>>>(h->d_tgtQ.p, h->d_omax.p);
         sub_omax_kernel<<<(unsigned)((nsub2 + 7) / 8), THREADS, 0, h->stream>>>(h->d_tgtQ.p, nsub2, h->d_omax_sub.p);
@@ -651,11 +731,11 @@ int launch_estep(cpd_ctx* h, const double* d_sigma2, const double* d_w, const do
     if (cull) { if (wgt) CPD_PASS2(true, true); else CPD_PASS2(true, false); }
     else { if (wgt) CPD_PASS2(false, true); else CPD_PASS2(false, false); }
 #undef CPD_PASS2
-    mark(h, 4);
+    mark(h, h->sev[4]);
     finalize2_kernel<<<blocks_for(h->m), THREADS, 0, h->stream>>>(h->d_state.p, d_sigma2, h->d_part2.p, h->d_slots2.p, (int)h->m, h->d_yc.p,
                                                                   d_ts, h->d_p1.p, h->d_pxc.p, h->d_mom_src.p);
-    mark(h, 5);
-    mark(h, 6);          // E-step-only callers end here; cpd_em_step / cpd_nonrigid_step record event 6 again after their M-step
+    mark(h, h->sev[5]);
+    mark(h, h->sev[6]);          // E-step-only callers end here; cpd_em_step / cpd_nonrigid_step record event 6 again after their M-step
     KCHECK();
     h->launches += 5;
     return CPD_OK;
@@ -674,9 +754,7 @@ int read_params(cpd_ctx* h, cpd_params* out) {
     for (int i = 0; i < 3; ++i) out->t[i] = (i < d) ? s.t[i] : 0.0;
     out->scale = s.scale;
     out->sigma2 = s.sigma2;
-    // a point reaches ~13.3 sigma (2^-127); culling can only pay once that is well inside the cloud
-    TRY(ensure_stats(h));
-    h->cull_active = h->extent > 0.0 && 13.3 * sqrt(out->sigma2) < 0.25 * h->extent;
+    TRY(decide_cull(h, out->sigma2));
     out->q = s.q;
     out->n_p = s.n_p;
     return CPD_OK;
@@ -761,9 +839,7 @@ extern "C" void cpd_destroy(cpd_ctx* h) {
     cudaSetDevice(h->device);
     cudaStreamSynchronize(h->stream);
     for (void* p : h->peer_ptr) if (p) cudaIpcCloseMemHandle(p);
-    if (h->sol_params && g_sol.DestroyParams) g_sol.DestroyParams(h->sol_params);
-    if (h->sol && g_sol.Destroy) g_sol.Destroy(h->sol);
-    delete h;                        // every buffer, pinned block, event and graph; the stream the handle created last
+    delete h;                        // every buffer, pinned block, event, graph and the solver; the stream the handle created last
 }
 
 extern "C" int cpd_set_source(cpd_ctx* h, const double* source, int64_t m) {
@@ -782,11 +858,10 @@ extern "C" int cpd_set_source(cpd_ctx* h, const double* source, int64_t m) {
         TRY(h->d_perm_src.alloc((size_t)m));
         TRY(h->d_outM.alloc((size_t)m * 3));
         h->prepared = false;
-        h->nr_ready = false;
+        if (h->nr.live()) h->nr.status = NrStatus::none;
     }
     TRY(ingest_cloud(h, source, m, 0, 0, nullptr, h->d_perm_src.p, h->d_yc.p));
-    h->bc_ready = false;                 // a BCPD loop starts from its own cpd_set_source + cpd_bcpd_begin
-    h->bc_stopped = false;
+    h->bc.status = BcStatus::none;       // a BCPD loop starts from its own cpd_set_source + cpd_bcpd_begin
     h->h_state.m = m;
     h->have_source = true;
     return CPD_OK;
@@ -822,7 +897,7 @@ extern "C" int cpd_set_target(cpd_ctx* h, const double* target, int64_t n_local,
 
 extern "C" int cpd_sigma2_init(cpd_ctx* h, double* sigma2) {
     if (!h || !sigma2) return fail(CPD_ERR_ARG, "null argument");
-    if (!h->have_source || !h->have_target) return fail(CPD_ERR_STATE, "source and target must both be set");
+    TRY(require_clouds(h));
     CU(cudaSetDevice(h->device));
     // target sums (summed over the ranks on the device), source sums, ONE read-back: a single host synchronisation
     double sx[4], sy[4];
@@ -858,16 +933,23 @@ extern "C" int cpd_set_state(cpd_ctx* h, int tf_kind, int update_scale, double w
     s.tf_kind = tf_kind;
     s.update_scale = update_scale ? 1 : 0;
     s.dim = d;
-    TRY(ensure_stats(h));
-    h->cull_active = h->extent > 0.0 && 13.3 * sqrt(init->sigma2) < 0.25 * h->extent;
-    h->have_state = true;
+    TRY(decide_cull(h, init->sigma2));
+    h->em = EmStatus::live;
+    h->nr.end("cpd_set_state ended the non-rigid loop of this handle: call cpd_nonrigid_*begin again");
     return upload_state(h);
 }
 
 namespace {
+// the refusal of an EM step without a live EM loop
+int em_check(cpd_ctx* h) {
+    if (h->em == EmStatus::none) return fail(CPD_ERR_STATE, "cpd_set_state has not been called");
+    if (h->em == EmStatus::ended)
+        return fail(CPD_ERR_STATE, "%s ended the rigid/affine EM loop of this handle: call cpd_set_state again", h->em_ended_by);
+    return CPD_OK;
+}
 // the launches of one fused EM iteration, in stream order (also what a graph capture records)
 int em_step_launches(cpd_ctx* h) {
-    TRY(launch_estep(h, &h->d_state.p->sigma2, &h->d_state.p->w, nullptr));
+    TRY(launch_estep(h, &h->d_state.p->sigma2, &h->d_state.p->w, nullptr, false));
     const int nbs = (int)blocks_for(h->m), nbt = (int)blocks_for(h->npad);
     if (h->d_p2p.p) {
         moments_p2p_kernel<<<1, 256, 0, h->stream>>>(h->d_state.p, h->d_mom_src.p, nbs, RM_SRC, h->d_mom_tgt.p, nbt, RM_TGT, h->d_mom.p,
@@ -882,7 +964,7 @@ int em_step_launches(cpd_ctx* h) {
         moments_kernel<1><<<1, 256, 0, h->stream>>>(h->d_state.p, h->d_mom_src.p, nbs, RM_SRC, h->d_mom_tgt.p, nbt, RM_TGT, h->d_mom.p);
         h->launches += 1;
     }
-    mark(h, 6);
+    mark(h, h->sev[6]);
     KCHECK();
     return CPD_OK;
 }
@@ -893,10 +975,10 @@ int em_step_launches(cpd_ctx* h) {
 // the kernels) and the ncclAllReduce variant of the multi-rank exchange (CPD_B200_NO_P2P=1); CPD_B200_NO_GRAPH=1 turns it off.
 extern "C" int cpd_em_step(cpd_ctx* h, cpd_params* out) {
     if (!h) return fail(CPD_ERR_ARG, "null handle");
-    if (!h->have_state) return fail(CPD_ERR_STATE, "cpd_set_state has not been called");
+    TRY(em_check(h));
     CU(cudaSetDevice(h->device));
 #ifndef CPD_HOST_EMU
-    const bool use_graph = h->graph_on && !h->profiling && !(h->comm && !h->d_p2p.p) && !h->wgt_on;
+    const bool use_graph = h->graph_on && !h->profiling && !(h->comm && !h->d_p2p.p);
 #else
     const bool use_graph = false;
 #endif
@@ -935,7 +1017,7 @@ extern "C" int cpd_em_step(cpd_ctx* h, cpd_params* out) {
 
 extern "C" int cpd_em_run(cpd_ctx* h, int maxiter, double tol, cpd_params* out, int* iters_run, double* trace) {
     if (!h || !out) return fail(CPD_ERR_ARG, "null argument");
-    if (!h->have_state) return fail(CPD_ERR_STATE, "cpd_set_state has not been called");
+    TRY(em_check(h));
     double q = h->h_state.q;
     int it = 0;
     cpd_params cur;
@@ -952,26 +1034,34 @@ extern "C" int cpd_em_run(cpd_ctx* h, int maxiter, double tol, cpd_params* out, 
     return CPD_OK;
 }
 
-extern "C" int cpd_estep(cpd_ctx* h, const double* t_source, double sigma2, double w, double* pt1, double* p1, double* px, double* n_p) {
-    if (!h || !t_source) return fail(CPD_ERR_ARG, "null argument");
-    if (!(sigma2 > 0.0)) return fail(CPD_ERR_ARG, "sigma2 must be positive, got %g", sigma2);
-    if (!(w >= 0.0 && w < 1.0)) return fail(CPD_ERR_ARG, "w must be in [0, 1), got %g", w);
-    if (!h->have_source || !h->have_target) return fail(CPD_ERR_STATE, "source and target must both be set");
-    CU(cudaSetDevice(h->device));
+namespace {
+// The stand-alone E-step at the caller's moved source, sigma2 and w (weighted: with the exponents bcpd_weights formed) into the
+// E-step's buffers, summed over the ranks
+int run_estep(cpd_ctx* h, const double* t_source, double sigma2, double w, bool weighted) {
     TRY(h->d_raw.reserve((size_t)h->m * 3));
     TRY(upload_cloud(h, t_source, h->m, h->d_raw.p));
     gather3_kernel<<<blocks_for(h->m), THREADS, 0, h->stream>>>(h->d_raw.p, h->d_perm_src.p, h->m, 0.0, 0.0, 0.0, h->d_ts.p);
     h->launches += 1;
-    TRY(ensure_stats(h));
-    h->cull_active = h->extent > 0.0 && 13.3 * sqrt(sigma2) < 0.25 * h->extent;
+    TRY(decide_cull(h, sigma2));
     h->pin.p->es[0] = sigma2;
     h->pin.p->es[1] = w;
     CU(cudaMemcpyAsync(&h->d_state.p->es_sigma2, h->pin.p->es, 2 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-    TRY(launch_estep(h, &h->d_state.p->es_sigma2, &h->d_state.p->es_w, h->d_ts.p));
+    TRY(launch_estep(h, &h->d_state.p->es_sigma2, &h->d_state.p->es_w, h->d_ts.p, weighted));
     if (h->comm) {
         TRY(allreduce(h, h->d_p1.p, (size_t)h->m));
         TRY(allreduce(h, h->d_pxc.p, (size_t)h->m * 3));
     }
+    return CPD_OK;
+}
+}  // namespace
+
+extern "C" int cpd_estep(cpd_ctx* h, const double* t_source, double sigma2, double w, double* pt1, double* p1, double* px, double* n_p) {
+    if (!h || !t_source) return fail(CPD_ERR_ARG, "null argument");
+    if (!(sigma2 > 0.0)) return fail(CPD_ERR_ARG, "sigma2 must be positive, got %g", sigma2);
+    if (!(w >= 0.0 && w < 1.0)) return fail(CPD_ERR_ARG, "w must be in [0, 1), got %g", w);
+    TRY(require_clouds(h));
+    CU(cudaSetDevice(h->device));
+    TRY(run_estep(h, t_source, sigma2, w, false));
     return cpd_last_estep(h, pt1, p1, px, n_p);
 }
 
@@ -1015,7 +1105,7 @@ extern "C" int cpd_bcpd_estep(cpd_ctx* h, const double* t_source, double scale, 
     if (!h || !t_source || !alpha || !sigma_diag) return fail(CPD_ERR_ARG, "null argument");
     if (!(sigma2 > 0.0)) return fail(CPD_ERR_ARG, "sigma2 must be positive, got %g", sigma2);
     if (!(w >= 0.0 && w < 1.0)) return fail(CPD_ERR_ARG, "w must be in [0, 1), got %g", w);
-    if (!h->have_source || !h->have_target) return fail(CPD_ERR_STATE, "source and target must both be set");
+    TRY(require_clouds(h));
     CU(cudaSetDevice(h->device));
     const long long m = h->m;
     bool any_weight = false;
@@ -1033,23 +1123,7 @@ extern "C" int cpd_bcpd_estep(cpd_ctx* h, const double* t_source, double scale, 
     CU(cudaMemcpyAsync(h->d_outM.p, alpha, (size_t)m * sizeof(double), cudaMemcpyHostToDevice, h->stream));
     CU(cudaMemcpyAsync(h->d_outM.p + m, sigma_diag, (size_t)m * sizeof(double), cudaMemcpyHostToDevice, h->stream));
     TRY(bcpd_weights(h, h->d_outM.p, h->d_outM.p + m, h->d_perm_src.p, h->d_bc_es.p));
-    TRY(h->d_raw.reserve((size_t)m * 3));
-    TRY(upload_cloud(h, t_source, m, h->d_raw.p));
-    gather3_kernel<<<blocks_for(m), THREADS, 0, h->stream>>>(h->d_raw.p, h->d_perm_src.p, m, 0.0, 0.0, 0.0, h->d_ts.p);
-    h->launches += 1;
-    TRY(ensure_stats(h));
-    h->cull_active = h->extent > 0.0 && 13.3 * sqrt(sigma2) < 0.25 * h->extent;
-    h->pin.p->es[0] = sigma2;
-    h->pin.p->es[1] = w;
-    CU(cudaMemcpyAsync(&h->d_state.p->es_sigma2, h->pin.p->es, 2 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-    h->wgt_on = true;
-    const int r = launch_estep(h, &h->d_state.p->es_sigma2, &h->d_state.p->es_w, h->d_ts.p);
-    h->wgt_on = false;
-    TRY(r);
-    if (h->comm) {
-        TRY(allreduce(h, h->d_p1.p, (size_t)m));
-        TRY(allreduce(h, h->d_pxc.p, (size_t)m * 3));
-    }
+    TRY(run_estep(h, t_source, sigma2, w, true));
     return cpd_last_estep(h, nu_d, nu, px, n_p);
 }
 
@@ -1062,18 +1136,11 @@ extern "C" int cpd_last_estep(cpd_ctx* h, double* pt1, double* p1, double* px, d
         CU(cudaMemcpyAsync(pt1, h->d_outN.p, (size_t)h->n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
         h->launches += 1;
     }
-    if (p1) {
-        scatter_kernel<<<blocks_for(h->m), THREADS, 0, h->stream>>>(h->d_p1.p, h->d_perm_src.p, h->m, 1, h->d_outM.p);
-        CU(cudaMemcpyAsync(p1, h->d_outM.p, (size_t)h->m * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-        CU(cudaStreamSynchronize(h->stream));      // d_outM is reused for px below
-        h->launches += 1;
-    }
+    if (p1) TRY(download_src(h, h->d_p1.p, 1, p1));
     if (px) {
         uncentre_px_kernel<<<blocks_for(h->m), THREADS, 0, h->stream>>>(h->d_state.p, h->d_p1.p, h->d_pxc.p, (int)h->m, h->d_px.p);
-        scatter_kernel<<<blocks_for(h->m), THREADS, 0, h->stream>>>(h->d_px.p, h->d_perm_src.p, h->m, 3, h->d_outM.p);
-        KCHECK();
-        h->launches += 2;
-        TRY(download_cloud(h, h->d_outM.p, h->m, px));
+        h->launches += 1;
+        TRY(download_src(h, h->d_px.p, 3, px));
     }
     if (n_p) {
         // n_p = sum(p1) (cpd.py:88): block partials of the (possibly all-reduced) p1
@@ -1090,19 +1157,9 @@ extern "C" int cpd_last_estep(cpd_ctx* h, double* pt1, double* p1, double* px, d
     return CPD_OK;
 }
 
-extern "C" int cpd_mstep(cpd_ctx* h, int tf_kind, int update_scale, const double* pt1, const double* p1, const double* px, double n_p,
-                         cpd_params* out) {
-    (void)n_p;   // recomputed as sum(p1), which is what the reference passes (cpd.py:88)
-    if (!h || !pt1 || !p1 || !px || !out) return fail(CPD_ERR_ARG, "null argument");
-    if (tf_kind != CPD_TF_RIGID && tf_kind != CPD_TF_AFFINE) return fail(CPD_ERR_ARG, "tf_kind %d not supported", tf_kind);
-    if (!h->have_source || !h->have_target) return fail(CPD_ERR_STATE, "source and target must both be set");
-    CU(cudaSetDevice(h->device));
-    TRY(prepare(h));
-    h->h_state.tf_kind = tf_kind;
-    h->h_state.update_scale = update_scale ? 1 : 0;
-    // only the two selectors: the rest of the device state may be ahead of the host mirror
-    CU(cudaMemcpyAsync(&h->d_state.p->tf_kind, &h->h_state.tf_kind, 2 * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-    // caller's order -> internal (Morton) order
+namespace {
+// a caller's E-step result (pt1, p1, px as cpd_estep returns them) into d_pt1, d_p1 and d_px, caller's order -> internal (Morton) order
+int upload_estep(cpd_ctx* h, const double* pt1, const double* p1, const double* px) {
     CU(cudaMemcpyAsync(h->d_outN.p, pt1, (size_t)h->n * sizeof(double), cudaMemcpyHostToDevice, h->stream));
     gather1_kernel<<<blocks_for(h->n), THREADS, 0, h->stream>>>(h->d_outN.p, h->d_perm_tgt.p, h->n, h->d_pt1.p);
     CU(cudaMemcpyAsync(h->d_outM.p, p1, (size_t)h->m * sizeof(double), cudaMemcpyHostToDevice, h->stream));
@@ -1110,7 +1167,26 @@ extern "C" int cpd_mstep(cpd_ctx* h, int tf_kind, int update_scale, const double
     TRY(h->d_raw.reserve((size_t)h->m * 3));
     TRY(upload_cloud(h, px, h->m, h->d_raw.p));
     gather3_kernel<<<blocks_for(h->m), THREADS, 0, h->stream>>>(h->d_raw.p, h->d_perm_src.p, h->m, 0.0, 0.0, 0.0, h->d_px.p);
+    KCHECK();
     h->launches += 3;
+    return CPD_OK;
+}
+}  // namespace
+
+extern "C" int cpd_mstep(cpd_ctx* h, int tf_kind, int update_scale, const double* pt1, const double* p1, const double* px, double n_p,
+                         cpd_params* out) {
+    (void)n_p;   // recomputed as sum(p1), which is what the reference passes (cpd.py:88)
+    if (!h || !pt1 || !p1 || !px || !out) return fail(CPD_ERR_ARG, "null argument");
+    if (tf_kind != CPD_TF_RIGID && tf_kind != CPD_TF_AFFINE) return fail(CPD_ERR_ARG, "tf_kind %d not supported", tf_kind);
+    TRY(require_clouds(h));
+    CU(cudaSetDevice(h->device));
+    TRY(prepare(h));
+    h->nr.end("cpd_mstep ended the non-rigid loop of this handle: call cpd_nonrigid_*begin again");
+    h->h_state.tf_kind = tf_kind;
+    h->h_state.update_scale = update_scale ? 1 : 0;
+    // only the two selectors: the rest of the device state may be ahead of the host mirror
+    CU(cudaMemcpyAsync(&h->d_state.p->tf_kind, &h->h_state.tf_kind, 2 * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    TRY(upload_estep(h, pt1, p1, px));
     const int nbs = (int)blocks_for(h->m), nbt = (int)blocks_for(h->n);
     centre_px_kernel<<<nbs, THREADS, 0, h->stream>>>(h->d_state.p, h->d_p1.p, h->d_px.p, (int)h->m, h->d_pxc.p);
     src_moments_api_kernel<<<nbs, THREADS, 0, h->stream>>>((int)h->m, h->d_yc.p, h->d_p1.p, h->d_pxc.p, h->d_mom_src.p);
